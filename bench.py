@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — prove-trace replay of the Halo2/KZG prover hot path on B200 (BASELINE.json metric: prove time (s) at k;
+"""bench.py — prove-trace replay of the Halo2/KZG prover hot path on H100 (BASELINE.json metric: prove time (s) at k;
 MSM G1 pairs/s and NTT Fr elts/s vs the HBM roofline).
 
 A "step" is ONE proof's worth of hot-path work (SURVEY.md §3.1 stages 1-9 minus synthesize / transcript, which stay on the
@@ -25,6 +25,10 @@ for a circuit of the shape named in `config.workload`, on synthetic seeded colum
                 inside the library on the launching stream.
   * `cpu_baseline` / `--impl reference`: the CPU restatement of halo2's Rayon algorithms (oracle/, "port") running the WHOLE
                 trace for real on the box's host cores (a persistent thread pool, every op instance executed, nothing extrapolated).
+--dump-outputs DIR: after the timed steps, what the last timed step returned to its caller (normalised commitments, evaluations,
+a seeded row sample of the quotient's coefficients and of the Kate quotients) is written as DIR/<name>.npy, float64 holding the
+exact 32-bit words of every limb, so that two builds can be compared output for output on identical seeded inputs.  With
+--gpus N > 1 the files hold what rank 0 computed: its share of the commitments, evaluations and Kate quotients, and the quotient.
 --simulate-rank-of N: ONE GPU executes rank 0's share of an N-way run (same deal, same kernels, exchanges skipped) so that a rank's
 per-step kernel list can be profiled without N GPUs; the line is marked SIMULATED and is not a bench value.
 N > 1 (torchrun): independent columns are dealt round-robin to ranks (strong scaling, no data-path collective inside an
@@ -32,6 +36,7 @@ op; one small all-gather of the commitments per step), timed as max over ranks; 
 process driving all N devices through the library's own multi-device host-pointer path (`in_process`).
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -113,11 +118,27 @@ def gate_program(m):
     return ev.QuotientProgram(value)
 
 
+DUMP_MAX_ROWS = 1 << 16      # rows kept per dumped array: 64 B per Fr row, so every dump stays far below 64 MB
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each uint64 limb array as DIR/<name>.npy: float64 holding its exact 32-bit words (lossless, < 2^53).  Arrays longer
+    than DUMP_MAX_ROWS keep a fixed seeded sample of rows (the same rows on every run), stored with their row indices."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype=np.uint64)
+        rows = np.arange(a.shape[0])
+        if a.shape[0] > DUMP_MAX_ROWS:
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], DUMP_MAX_ROWS, replace=False))
+            np.save(os.path.join(out_dir, name + "_rows.npy"), rows.astype(np.float64))
+        np.save(os.path.join(out_dir, name + ".npy"), a[rows].view(np.uint32).astype(np.float64))
+
+
 class ClockSampler(threading.Thread):
     """Samples SM clocks / throttle reasons while the timed regions run: ONE long-lived `nvidia-smi -lms 100` process (started
     before the warm-up so its start-up cost is outside the timed region); rows are stamped on arrival and only those that fall
     inside a marked region are summarised."""
-    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, device):
         super().__init__(daemon=True)
@@ -127,6 +148,7 @@ class ClockSampler(threading.Thread):
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.device), "--query-gpu=" + self.Q, "--format=csv,noheader,nounits", "-lms", "100"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.proc.terminate)        # the sampler never outlives bench.py, even when a leg fails
             for line in self.proc.stdout:
                 parts = [x.strip() for x in line.strip().split(",")]
                 if len(parts) >= 8:
@@ -152,7 +174,7 @@ class ClockSampler(threading.Thread):
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": float(inside[0][2]), "power_w_max": max(float(r[3]) for r in inside),
-                "reasons": sorted(reasons), "samples": len(inside)}
+                "power_limit_w": float(inside[0][8]) if len(inside[0]) > 8 else None, "reasons": sorted(reasons), "samples": len(inside)}
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -240,7 +262,9 @@ def run_b200(args):
     assert world == 1 << log_g and world <= (1 << tr["ext_bits"]), "quotient stage: world must be a power of two <= 2^ext_bits"
     N_ext = 1 << ext_k
     slab = N_ext // world
-    group = QUOTIENT_GROUP if ext_k <= 23 else 16
+    # coset columns per evaluate_h group: at ext_k >= 24 a group of 2^ext_k-row cosets (plus its NTT scratch) must fit beside the
+    # resident column pool and window tables on an 80 GB H100
+    group = QUOTIENT_GROUP if ext_k <= 23 else 4
     programs = {}
     d_ext = 1 << tr["ext_bits"]
     tinv_local = np.ascontiguousarray(np.stack([dom.t_evaluations[(rank + world * t) % d_ext] for t in range(max(1, d_ext // world))]))
@@ -351,6 +375,7 @@ def run_b200(args):
             if m not in programs:
                 programs[m] = gate_program(m)
             h = ev.evaluate_h_device(programs[m], slabs + [h], k, ext_k - log_g)
+            del ext_my, slabs        # the next group's coset NTT may reuse this group's memory
         dev.scale_cycle(h, tinv_local)
         if world > 1:
             parts = [torch.empty_like(h) for _ in range(world)]
@@ -376,6 +401,8 @@ def run_b200(args):
         _g += _count
 
     evals = []
+    last = {}          # --dump-outputs: the last step's quotient coefficients and Kate quotients (references, no copy)
+    keep_h = (lambda h_: last.__setitem__("quotient", h_)) if args.dump_outputs else None
     npolys_total = tr["advice"] + tr["fixed"] + tr["perm_cols"] + tr["perm_z"] + 2 * tr["lookups"] + 1 + tr["quotient_pieces"]
     lin_scalars = np.ascontiguousarray(np.tile(xs, (npolys_total // ncols + 1, 1))[:npolys_total])
 
@@ -426,7 +453,7 @@ def run_b200(args):
                     if fut is not None:
                         fut.result()                  # the side thread has ENQUEUED everything (its done event is recorded); no device sync
                         fut = None
-                    quotient_stage(lambda j: cols_[j % ncols], None, early=two)
+                    quotient_stage(lambda j: cols_[j % ncols], keep_h, early=two)
                 elif kind == "eval":
                     evals.append(dev.eval_batch(v, xs[:b]))
                 elif kind == "lincomb":
@@ -436,6 +463,8 @@ def run_b200(args):
                 elif kind == "kate_division":
                     for i in range(b):
                         dev.kate_division(v[i], xs[i], out=out_n[i][: n - 1])
+                    if args.dump_outputs:
+                        last["kate"] = out_n[:b, : n - 1]          # the rows this rank computed in this step
                 done += b
         pts = torch.cat(commits) if commits else torch.zeros((0, 16), dtype=torch.int64, device="cuda")
         if world > 1 and not sim:
@@ -625,12 +654,15 @@ def run_b200(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        step_device()
+        pts_last = step_device()
     e1.record()
     issue_ms = (time.time() - t_reg0) * 1e3 / args.steps     # host time to ENQUEUE a step (close to ms_per_step means the host issue rate is the limiter)
     barrier()
     sampler.mark(t_reg0, time.time())
     launches = nat.launch_count() - l0
+    if args.dump_outputs and rank == 0:          # the later legs re-run the trace and overwrite these buffers
+        dump_outputs(args.dump_outputs, {"commitments": dev.normalize(pts_last), "evaluations": dev.to_host(torch.cat(evals)),
+                                         "quotient_coeffs": dev.to_host(last["quotient"]), "kate_quotients": dev.to_host(last.get("kate", out_n[:0, : n - 1]).reshape(-1, 4))})
     ms_dev = max_over_ranks(e0.elapsed_time(e1)) / args.steps
     # ---- same steps again with per-kernel-class CUDA events (roofline leg; not part of `value`)
     nat.check(L.b200_profile_enable(1))
@@ -701,8 +733,8 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "H100 SXM data sheet (3.35 TB/s, not measured)"
     # dominant kernel: MSM bucket accumulation.  Algorithmic bytes = 32 B scalar + 64/b B shared base per pair
     # (SURVEY.md §8d), per launch = pairs in that launch; summed over the step and divided by the summed kernel time.
     my_msm_cols = 0
@@ -716,22 +748,15 @@ def run_b200(args):
     launch_cols = my_msm_cols * args.steps / max(acc_cnt, 1)
     alg_bytes_per_launch = launch_cols * n * (32.0 + 64.0 / max(launch_cols, 1.0))
     achieved = alg_bytes_per_launch / ((acc_ms / max(acc_cnt, 1)) * 1e-3) / 1e9 if acc_ms > 0 else 0.0
-    # DRAM traffic of the dominant kernel from the committed `ncu --set full` capture of this same command (k = 17 only)
-    traffic = None
-    try:
-        cap_path = os.path.join(ROOT, "profiles", "r02_ncu_full_bench_step_k17.json")
-        if not os.path.exists(cap_path):
-            cap_path = os.path.join(ROOT, "profiles", "r01_ncu_full_bench_step_k17.json")
-        cap = json.load(open(cap_path))["k_accumulate"]
-        if k == 17 and tname == "conv2d_mnist" and world == 1:
-            rd, wr = cap["dram__bytes_read.sum"]["per_launch"], cap["dram__bytes_write.sum"]["per_launch"]
-            traffic = int(sum(rd + wr) * 1e9 / len(rd))
-    except Exception:
-        pass
+    # integer-multiply roofline: 64 32-bit product words per clock per SM (the IMAD rate of compute capability 9.0) at the
+    # card's maximum SM clock as nvidia-smi reports it
+    sms = torch.cuda.get_device_properties(local).multi_processor_count
+    peak_words = sms * 64 * clocks["sm_max_mhz"] * 1e6 if clocks.get("sm_max_mhz") else None
     msm_ms = prof["msm_total"][0] / args.steps
     ntt_ms = prof["ntt"][0] / args.steps
     line = {
         "metric": "prove_time_s", "value": round(ms_dev / 1e3, 6), "unit": "s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
+        "gpu": torch.cuda.get_device_name(local),
         "ms_per_step": round(ms_dev, 3), "higher_is_better": False, "scaling": "strong", "vs_baseline": None,
         "dtype": "u32 limbs (254-bit Montgomery integers mod BN254 r/p)", "data": "synthetic",
         "config": make_config(k, tname),
@@ -747,16 +772,16 @@ def run_b200(args):
         "gpu_launches": int(launches),
         "clocks": clocks,
         "roofline": {"kernel": "k_accumulate (MSM bucket accumulation)", "bound": "hbm", "achieved": round(achieved, 2), "peak": hbm_peak, "unit": "GB/s",
-                     "frac": round(achieved / hbm_peak, 5), "traffic": traffic, "peak_source": peak_src,
+                     "frac": round(achieved / hbm_peak, 5), "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": int(alg_bytes_per_launch), "avg_launch_ms": round(acc_ms / max(acc_cnt, 1), 4),
                      "kernel_share_of_step": round(acc_ms / args.steps / ms_dev, 4) if ms_dev > 0 else None,
-                     "issue_bound": {"what": "the integer-multiply roofline of the SM: 16 32-bit product words / clk / sub-partition = 148 x 64 x 1.965 GHz = 18.6 T words/s (IMAD = 1 word, IMAD.WIDE = 2 words, "
-                                             "carries free; profiles/r02_pipe_probe2_carry_cost.txt).  One bucket addition (XYZZ += affine) = 6 multiplications x 264 words + one two-product multiplication "
-                                             "with a single reduction (392) + 2 squarings of 36 products (208 each) = 2392 words",
+                     "issue_bound": {"what": "the integer-multiply roofline of the SM: 16 32-bit product words / clk / sub-partition = %d SMs x 64 x the maximum SM clock "
+                                             "(IMAD = 1 word, IMAD.WIDE = 2 words, carries free).  One bucket addition (XYZZ += affine) = 6 multiplications x 264 words + one "
+                                             "two-product multiplication with a single reduction (392) + 2 squarings of 36 products (208 each) = 2392 words" % sms,
                                      "adds_per_s": round(my_msm_cols * n * win / (acc_ms / args.steps * 1e-3), 1) if acc_ms > 0 else None,
                                      "words_per_s": round(my_msm_cols * n * win * 2392 / (acc_ms / args.steps * 1e-3), 1) if acc_ms > 0 else None,
-                                     "peak_words_per_s": 148 * 64 * 1.965e9,
-                                     "frac": round(my_msm_cols * n * win * 2392 / (acc_ms / args.steps * 1e-3) / (148 * 64 * 1.965e9), 4) if acc_ms > 0 else None},
+                                     "peak_words_per_s": peak_words,
+                                     "frac": round(my_msm_cols * n * win * 2392 / (acc_ms / args.steps * 1e-3) / peak_words, 4) if acc_ms > 0 and peak_words else None},
                      "note": "integer-issue bound (254-bit modular arithmetic), not HBM bound: see DESIGN.md"},
         "msm_pairs_per_s": round(pairs / world / (msm_ms * 1e-3), 1) * world if msm_ms > 0 else None,
         "ntt_elts_per_s": round(ntt_elts / world / (ntt_ms * 1e-3), 1) * world if ntt_ms > 0 else None,
@@ -793,7 +818,7 @@ class CpuTrace:
         self.cols = [orc.gen_scalars(self.n, seed=6 + i) for i in range(self.ncols)]
         self.xs = orc.gen_scalars(self.ncols, seed=7)
         self.one = orc.fr_one()
-        self.group = QUOTIENT_GROUP if self.ext_k <= 23 else 16
+        self.group = QUOTIENT_GROUP if self.ext_k <= 23 else 4
         self.programs = {}
         self.per_op = {}
 
@@ -856,15 +881,14 @@ def cpu_baseline(k, tname):
 
 
 def run_reference(args):
-    """The reference arm: the CPU port executing whole trace steps in a real loop.  A k = 17 step takes tens of seconds on 128
-    cores, so the loop is bounded by --cpu-budget seconds of wall time: at most `--warmup` (capped at 1) untimed + `--steps` timed
-    steps, never fewer than one timed step; `steps` / `warmup` in the line are what actually ran."""
+    """The reference arm: the CPU port executing whole trace steps in a real loop: exactly `--steps` timed steps (at least one).
+    A k = 17 step takes tens of seconds even on many cores, so at most one untimed warm-up step runs, and when that step alone takes
+    more than half of --cpu-budget it is counted as the first timed step instead of being discarded; `warmup` in the line says which."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
     k = args.k
     tname = args.trace or CONFIG_FOR_K.get(k, "conv2d_mnist")
-    t_all = time.perf_counter()
     ct = CpuTrace(k, tname)
     budget = max(args.cpu_budget, 1.0)
     warm = 0
@@ -876,13 +900,11 @@ def run_reference(args):
             vals.append(first)
             warm = 0
     while len(vals) < max(1, args.steps):
-        if vals and (time.perf_counter() - t_all) + 1.1 * max(vals) > budget:
-            break
         vals.append(ct.step())
     v = sum(vals) / len(vals)
     base = {"value": round(v, 4), "unit": "s", "cores": ct.threads, "kind": "port",
             "sample": "%d whole trace step(s) timed after %d warm-up step(s), every op instance executed (restated halo2 algorithms, oracle/bn254_oracle.c; "
-                      "not the Rust binary); requested --steps %d --warmup %d, bounded by --cpu-budget %.0f s" % (len(vals), warm, args.steps, args.warmup, budget),
+                      "not the Rust binary); requested --steps %d --warmup %d, warm-up affordable within --cpu-budget %.0f s" % (len(vals), warm, args.steps, args.warmup, budget),
             "per_step_s": [round(x, 3) for x in vals], "per_op_s": ct.per_op}
     line = {"impl": "reference", "metric": "prove_time_s", "value": round(v, 4), "unit": "s", "n_gpus": args.gpus, "steps": len(vals), "warmup": warm,
             "ms_per_step": round(v * 1e3, 1), "higher_is_better": False, "scaling": "strong", "vs_baseline": None,
@@ -901,14 +923,17 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--k", type=int, default=17)
     ap.add_argument("--trace", default=None, choices=[None] + list(TRACES))
-    ap.add_argument("--cpu-budget", type=float, default=150.0, help="--impl reference: wall-clock bound of the whole run in seconds")
+    ap.add_argument("--cpu-budget", type=float, default=150.0, help="--impl reference: a warm-up step longer than half of this many seconds counts as the first timed step")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity-gate", action="store_true", help="skip the oracle comparison of the timed inputs (profiling runs only; the line says parity_checked: false)")
     ap.add_argument("--no-host-pointer-e2e", action="store_true")
     ap.add_argument("--profile-one-step", action="store_true", help="setup + one device step only (for ncu launch lists)")
     ap.add_argument("--no-overlap", action="store_true", help="single-stream schedule (trace order), for A/B against the two-stream schedule")
     ap.add_argument("--simulate-rank-of", type=int, default=0, help="profiling aid: run rank 0's share of an N-way run on ONE GPU (collectives skipped); the line is marked SIMULATED")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write what the last timed step returned as DIR/<name>.npy (float64 words of the limbs; rank 0's share when --gpus > 1)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs writes the GPU arm's outputs; --impl reference has none to write")
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
     if args.impl == "reference":

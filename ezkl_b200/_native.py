@@ -1,6 +1,6 @@
 """ctypes binding of libezkl_b200.so (the C ABI in include/ezkl_b200.h).
 
-There is no fallback: if the shared library is missing, or b200_init finds no sm_100 device, the error is raised to the
+There is no fallback: if the shared library is missing, or b200_init finds no sm_90 device, the error is raised to the
 caller.  Arrays are numpy uint64 in the wire format (Fr -> [...,4], G1Affine -> [...,8], G1 Jacobian -> [...,12],
 XYZZ -> [...,16]); device-resident entry points take raw device pointers (ints), e.g. torch ``tensor.data_ptr()``.
 """

@@ -25,6 +25,17 @@ namespace b200 {
 // ---- configuration: the environment is read once, in b200_init --------------------------------------------------------------
 static Config g_cfg;
 const Config& config() { return g_cfg; }
+int sm_count() {
+    static std::atomic<int> cache[64];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+    int v = cache[dev].load(std::memory_order_relaxed);
+    if (v == 0) {
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
+        cache[dev].store(v, std::memory_order_relaxed);
+    }
+    return v;
+}
 static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
 static void read_config() {
     Config c;
@@ -178,7 +189,7 @@ static size_t call_budget() {
 static inline Fr as_fr(const b200_fr* p) { Fr r; memcpy(&r, p, sizeof r); return r; }
 
 // ---- large host <-> device copies of PAGEABLE caller memory (what a Rust Vec<Fr> is) ------------------------------------------------
-// cudaMemcpyAsync from pageable memory runs at 6-7 GB/s on this box (one driver thread copying into its own staging buffer).  Here the
+// cudaMemcpyAsync from pageable memory is limited by one driver thread copying into its own staging buffer.  Here the
 // copy is cut into 16 MiB chunks that four host threads move into a pinned bounce buffer while the DMA engine drains the other one, so
 // the PCIe link (Gen5 x16) is fed at memcpy-pool speed.  Small copies keep the plain path.
 static constexpr size_t BOUNCE_BYTES = (size_t)16 << 20;
@@ -463,7 +474,7 @@ static int init_devices(const int* ids, int n) {
         B200_CHECK(device < count, -1, "b200_init: device %d >= device count %d", device, count);
         cudaDeviceProp prop;
         B200_CUDA(cudaGetDeviceProperties(&prop, device));
-        B200_CHECK(prop.major == 10, -2, "b200_init: device %d is sm_%d%d; this library carries sm_100a code only", device, prop.major, prop.minor);
+        B200_CHECK(prop.major == 9 && prop.minor == 0, -2, "b200_init: device %d is sm_%d%d; this library carries sm_90a code only", device, prop.major, prop.minor);
         B200_CUDA(cudaSetDevice(device));
         B200_CUDA(cudaFree(0));
         g_devs[s].id = device;

@@ -83,7 +83,7 @@ struct StagingRing {
 // Process-wide tuning knobs, read from the environment ONCE in b200_init (never on a launch path).
 struct Config {
     size_t ws_budget_call = 0;      // B200_WS_BUDGET_MB: fixed per-call scratch budget (tests use it to force the batch-split paths); 0 = derive
-    size_t ws_budget_total = (size_t)48 << 30;   // scratch the library may hold across all calling threads of a device
+    size_t ws_budget_total = (size_t)24 << 30;   // scratch the library may hold across all calling threads of a device (of an 80 GB H100)
     int ntt_v1 = 0;                 // B200_NTT_V=1: radix-2 shared-memory pass everywhere
     int ntt_logg = -1;              // B200_NTT_LOGG
     int ntt_threads = 0;            // B200_NTT_THREADS (v1 pass)
@@ -94,6 +94,8 @@ struct Config {
     int shard_min_logn = 22;        // B200_SHARD_MIN_LOGN: a single transform of at least this size is sharded across the devices
 };
 const Config& config();
+// Streaming multiprocessors of the current device (132 on an H100 SXM); grids are sized in multiples of it.
+int sm_count();
 
 // Optional device-side timing of kernel classes with CUDA events on the launching stream (bench.py's roofline leg).
 enum ProfClass { PROF_MSM_ACCUMULATE = 0, PROF_MSM_TOTAL = 1, PROF_NTT = 2, PROF_POLY = 3, PROF_MSM_RECODE = 4, PROF_MSM_TAIL = 5, PROF_QUOTIENT = 6, PROF_NCLASS = 7 };

@@ -1,8 +1,7 @@
 // ec_coop.cuh — four-lane cooperative XYZZ addition / doubling for the latency-bound tail of the MSM (bucket reduction, final sums).
 //
-// The tail is a chain of ~50-100 DEPENDENT group operations per column with little parallelism (ncu: 1.68 ms for a launch whose
-// multiplications would take 0.8 ms at the pipe's throughput; a lone warp needs ~5 us per addition because its 14 multiplications run
-// back to back).  Here the four lanes of a quad hold identical copies of the operands and each computes ONE of the independent products
+// The tail is a chain of ~50-100 DEPENDENT group operations per column with little parallelism (a lone warp pays the
+// latency of its 14 multiplications back to back on every addition, about twice their throughput cost).  Here the four lanes of a quad hold identical copies of the operands and each computes ONE of the independent products
 // of a formula level, the products are exchanged with quad-wide shuffles, and the cheap additions are done redundantly by all four:
 // an addition is 4 multiplication levels deep instead of 14 (doubling: 3 instead of 9), at 14 of 16 (10 of 12) lane-multiplications
 // of useful work.  Results are bit-identical to g1_add / g1_dbl (same formulas, exact arithmetic); every lane of the quad returns the

@@ -8,7 +8,7 @@ compared with Python bigint arithmetic BEFORE the header is written (``python fp
 
 Multiplication = operand-scanning Montgomery (CIOS) with the even/odd split accumulator: products a[j]*b_i for even
 j tile limbs (0,1),(2,3).. and for odd j tile (1,2),(3,4).., so each row is two independent chains of
-(lo,hi) pairs that ptxas can fuse into IMAD.WIDE.U32(.X) on sm_100a.  Modulus limbs are literal immediates.
+(lo,hi) pairs that ptxas can fuse into IMAD.WIDE.U32(.X) on sm_90a.  Modulus limbs are literal immediates.
 """
 import random
 import sys

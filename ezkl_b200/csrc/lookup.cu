@@ -78,7 +78,8 @@ int lookup_multiplicities_run(const Fr* d_table, size_t n_table, const Fr* const
     B200_CUDA(cudaMemsetAsync(counts, 0, sizeof(uint32_t) * n_table + 16, st));
     k_lk_build<<<div_up(n_table, 256), 256, 0, st>>>(d_table, (uint32_t)n_table, slots, cap - 1);
     if (n_rows) {
-        const unsigned gx = div_up(n_rows, 256) > 148u * 8u ? 148u * 8u : div_up(n_rows, 256);
+        const unsigned gmax = (unsigned)sm_count() * 8u;
+        const unsigned gx = div_up(n_rows, 256) > gmax ? gmax : div_up(n_rows, 256);
         k_lk_count<<<dim3(gx, (unsigned)n_inputs), 256, 0, st>>>(d_table, slots, cap - 1, d_inputs, (uint32_t)n_rows, counts, missing);
     }
     k_lk_finish<<<div_up(n_table, 256), 256, 0, st>>>(counts, (uint32_t)n_table, d_m);

@@ -1,4 +1,4 @@
-// msm.cu — BN254 G1 multi-scalar multiplication for sm_100a (Pippenger buckets over a window-precomputed table).
+// msm.cu — BN254 G1 multi-scalar multiplication for sm_90a (Pippenger buckets over a window-precomputed table).
 //
 // Replaces halo2_proofs arithmetic.rs best_multiexp / ParamsKZG::{commit, commit_lagrange} (UPSTREAM; in-tree
 // callers /root/reference/src/circuit/modules/polycommit.rs:71 and create_proof at src/pfsys/mod.rs:456).
@@ -456,8 +456,8 @@ int g1_sum_run(const G1Xyzz* d_points, size_t groups, size_t count, G1Xyzz* d_ou
 
 // ---------------------------------------------------------------------------------------------------------
 static uint32_t pick_cap(size_t total_entries) {
-    // aim for >= ~4 chunks per resident thread slot (148 SMs x 512 threads), chunk length a power of two in [16, 512]
-    size_t target = total_entries / ((size_t)148 * 512 * 4);
+    // aim for >= ~4 chunks per resident thread slot (SMs x 512 threads), chunk length a power of two in [16, 512]
+    size_t target = total_entries / ((size_t)sm_count() * 512 * 4);
     uint32_t cap = 16;
     while (cap < 512 && cap < target) cap <<= 1;
     return cap;
@@ -488,7 +488,7 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     // fix-up and a block tree).  Large batches are work bound: 32 buckets per thread, 256-thread CTAs.  Small batches are bound by the
     // LATENCY of that dependent chain (a lone warp needs ~7.5 us per group addition, about 1000 cycles per field multiplication, twice its
     // throughput cost), so fewer buckets per thread and more, smaller CTAs win until the extra threads' fix-ups and tree levels cost more
-    // than the shorter chain saves.  The table is the measured optimum per total bucket count (profiles/r02_msm_tail_sweep.txt).
+    // than the shorter chain saves.  The table is the optimum per total bucket count of the sweep in tools/bench_msm_tail_sweep.py.
     const size_t all_buckets = (size_t)batch * nb;
     uint32_t reduce_m = REDUCE_M_MAX, reduce_threads = TREE_THREADS;
     if (all_buckets <= ((size_t)1 << 15)) { reduce_m = 4; reduce_threads = 128; }
@@ -536,17 +536,18 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     ProfScope ps_total(PROF_MSM_TOTAL, st);
     B200_CUDA(cudaMemsetAsync(hist, 0, counts_words * 4, st));
     if (prof_enabled()) prof_mark(PROF_MSM_RECODE, st, true);
-    const unsigned dig_blocks = min(div_up(n, 256), 148u * 8u);
+    const unsigned sms = (unsigned)sm_count();
+    const unsigned dig_blocks = min(div_up(n, 256), sms * 8u);
     dim3 gd(dig_blocks, batch);
     k_digits<false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr);
     k_scan_buckets<<<batch, 1024, 0, st>>>(hist, offs, chunk_offs, nb, cap, skew);
     k_digits<true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew);
     k_fill_chunks<<<dim3(div_up(nb, 256), batch), 256, (cap + 1) * 4, st>>>(offs, chunk_offs, nb, cap, chunk_start, chunk_len, chunk_stride, len_hist, heavy, heavy_stride);
     k_len_offsets<<<batch, 32, 0, st>>>(len_hist, len_offs, cap);
-    const unsigned ch_blocks = min(div_up(chunk_stride, 256), 148u * 8u);
+    const unsigned ch_blocks = min(div_up(chunk_stride, 256), sms * 8u);
     k_order_chunks<<<dim3(ch_blocks, batch), 256, 0, st>>>(chunk_len, chunk_stride, chunk_offs, nb, len_offs, len_cursor, cap, order);
     if (prof_enabled()) prof_mark(PROF_MSM_RECODE, st, false);
-    const unsigned acc_blocks = min(div_up(chunk_stride, 128), 148u * 16u);
+    const unsigned acc_blocks = min(div_up(chunk_stride, 128), sms * 16u);
     {
         ProfScope ps(PROF_MSM_ACCUMULATE, st);
         k_accumulate<<<dim3(acc_blocks, batch), 128, 0, st>>>(t.d_table, ents, ent_stride, chunk_start, chunk_len, order, chunk_stride, chunk_offs, nb, chunk_sums);

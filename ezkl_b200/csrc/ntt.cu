@@ -1,4 +1,4 @@
-// ntt.cu — BN254 Fr number-theoretic transform for sm_100a.
+// ntt.cu — BN254 Fr number-theoretic transform for sm_90a.
 //
 // Replaces halo2_proofs arithmetic.rs best_fft and the EvaluationDomain transforms built on it (lagrange_to_coeff,
 // coeff_to_extended, extended_to_coeff; UPSTREAM poly/domain.rs — in-tree user /root/reference/src/circuit/modules/
@@ -348,7 +348,8 @@ static bool plan_pass_v2(PassArgs& a, uint64_t lines, int batch, uint32_t* threa
     if (a.logm < 2 || cfg.ntt_v1) return false;
     uint32_t log_g = a.logm >= 10 ? 0 : 10 - a.logm;
     if (cfg.ntt_logg >= 0) log_g = (uint32_t)cfg.ntt_logg;
-    while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < 296)) --log_g;
+    const uint64_t min_ctas = 2 * (uint64_t)sm_count();
+    while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < min_ctas)) --log_g;
     while (log_g > 0 && (a.logm + log_g > 10)) --log_g;
     if (a.logm + log_g < 7) return false;       // fewer than 32 quads: not worth a CTA
     a.log_g = log_g;
@@ -371,7 +372,8 @@ static int launch_pass_v1(PassArgs& a, uint64_t lines, int batch, cudaStream_t s
     // lines per CTA: largest G in {4,2,1} that still yields >= 2 CTAs per SM (and fits shared memory)
     const Config& cfg = config();
     uint32_t log_g = 2;
-    while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < 296)) --log_g;
+    const uint64_t min_ctas = 2 * (uint64_t)sm_count();
+    while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < min_ctas)) --log_g;
     while (log_g > 0 && (((size_t)1 << (a.logm + log_g)) + ((size_t)1 << a.logm) / 2) * 32 > 200 * 1024) --log_g;
     if (cfg.ntt_logg >= 0) { uint32_t v = (uint32_t)cfg.ntt_logg; while (v > 0 && (1u << v) > a.inner_cnt) --v; log_g = v; }
     a.log_g = log_g;

@@ -1,4 +1,4 @@
-// poly.cu — batched column-polynomial kernels over BN254 Fr for sm_100a.
+// poly.cu — batched column-polynomial kernels over BN254 Fr for sm_90a.
 //
 // Replaces the CPU `parallelize` loops of halo2_proofs (UPSTREAM arithmetic.rs / poly.rs / poly/domain.rs):
 //   Polynomial +,-,* and scalar ops, distribute_powers_zeta, divide_by_vanishing_poly, eval_polynomial,
@@ -42,7 +42,7 @@ __global__ void __launch_bounds__(256) k_poly_lincomb(const Fr* const* __restric
     }
 }
 
-static unsigned ew_grid(size_t n) { unsigned g = div_up(n, 256); return g > 148u * 16u ? 148u * 16u : (g ? g : 1); }
+static unsigned ew_grid(size_t n) { const unsigned gmax = (unsigned)sm_count() * 16u; unsigned g = div_up(n, 256); return g > gmax ? gmax : (g ? g : 1); }
 
 int poly_binary(int op, const Fr* a, const Fr* b, const Fr* h_s, Fr* out, size_t n, cudaStream_t st) {
     if (n == 0) return 0;

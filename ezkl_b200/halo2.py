@@ -1,4 +1,4 @@
-"""Host-side mirror of the halo2 interfaces on the prover hot path, executing on the B200 through the C ABI.
+"""Host-side mirror of the halo2 interfaces on the prover hot path, executing on the H100 through the C ABI.
 
 Same names, argument meaning and error behaviour as the reference's dependency (UPSTREAM halo2_proofs 0.3.0 @
 zkonduit/halo2#01c88842, not vendored; ezkl call sites cited per function), so the parity tests read like the reference's

@@ -1,7 +1,7 @@
-"""One-process-per-GPU sharding of the prover hot path over torch.distributed (NCCL over NVLink on the B200 box; gloo on
+"""One-process-per-GPU sharding of the prover hot path over torch.distributed (NCCL over NVLink between H100s; gloo on
 CPU for the host-logic tests).
 
-The reference has no multi-GPU layer at all (SURVEY.md §2.3); this is the B200-native addition the north star asks for:
+The reference has no multi-GPU layer at all (SURVEY.md §2.3); this is the multi-GPU addition the north star asks for:
   * column level  — a proof is ~100 independent MSM(n) and several hundred independent NTTs: `column_owner` deals whole
     columns to ranks, the SRS table is replicated, results are all-gathered (96 B per commitment).  No data-path
     collective inside an op.

@@ -1,5 +1,5 @@
 /*
- * ezkl_b200.h — C ABI of libezkl_b200.so, the Blackwell (sm_100a) proving backend for ezkl's Halo2/KZG prover.
+ * ezkl_b200.h — C ABI of libezkl_b200.so, the Hopper (sm_90a, H100) proving backend for ezkl's Halo2/KZG prover.
  *
  * This is the drop-in boundary (SURVEY.md §8b): the entry points a Rust `mod b200;` inside the halo2 fork binds in place
  * of `mod icicle;` behind cfg(feature = "gpu-accelerated") (/root/reference/Cargo.toml:259), so that
@@ -9,13 +9,13 @@
  * Conventions
  *   - return 0 = ok, < 0 = error (-1 bad argument, -2 CUDA failure, -3 not initialised); message via b200_last_error()
  *     (thread-local).  Nothing throws or aborts across the boundary; there is NO CPU fallback — without a usable
- *     sm_100 device every compute entry point fails with -2/-3.
+ *     sm_90 device every compute entry point fails with -2/-3.
  *   - the caller owns every host pointer for the duration of the call only; the library never frees caller memory.
  *   - Fr / Fq: 4 x u64 little-endian limbs in Montgomery form, exactly halo2curves' in-memory representation
  *     (zero-copy from &[Fr]).  G1 affine = {x, y} 64 B, identity = (0,0).  G1 Jacobian = {x, y, z} 96 B, identity z = 0.
  *   - every call is synchronous with respect to its host buffers and re-entrant: each calling thread gets its own CUDA
  *     stream and scratch arena per device (halo2 commits / transforms columns from Rayon worker threads).  The scratch
- *     the library holds is bounded process-wide (B200_WS_TOTAL_MB, default 48 GiB per device, divided among the calling
+ *     the library holds is bounded process-wide (B200_WS_TOTAL_MB, default 24 GiB per device, divided among the calling
  *     threads), released when a calling thread exits and at b200_shutdown, which first waits for calls in flight.
  *   - a process may own 1, 2, 4 or 8 devices (b200_init_multi).  Host-pointer entry points then use all of them: columns
  *     of a batch are dealt over the devices, a single MSM is split by base range, a single transform of >= 2^22 elements is

@@ -1,19 +1,23 @@
 #!/usr/bin/env python
 """Regenerates tests/golden/* from the reference's own checked-in fixtures.
 
-Run in the build container only (reads /root/reference, which does not exist on the GPU box):
-    python tests/golden/make_golden.py
+Needs a checkout of zkonduit/ezkl; EZKL_ASSETS names its tests/assets directory.  The tests read only the outputs.
 
-Inputs (reference fixtures, SURVEY.md Appendix B):
-  /root/reference/tests/assets/kzg     ParamsKZG::write output for k=6 (what src/pfsys/srs.rs:40-47 reads)
-  /root/reference/tests/assets/pk.key  ProvingKey::write (RawBytes), read by src/pfsys/mod.rs:615
+Inputs (the reference's fixtures, SURVEY.md Appendix B):
+  ASSETS/kzg                        ParamsKZG::write output for k=6 (what src/pfsys/srs.rs:40-47 reads)
+  ASSETS/pk.key                     ProvingKey::write (RawBytes), read by src/pfsys/mod.rs:615
+  ASSETS/proof.json                 a proof the Rust prover made for the k=6 circuit of pk.key
 
 Outputs:
   tests/golden/kzg_k6.srs           the 8452-byte SRS data fixture, verbatim (data, not source)
+  tests/golden/reference_proof_k6.bin  the `proof` bytes of proof.json, verbatim
+  tests/golden/pk_k6_primary.npz    the sections of pk.key that keygen does not derive: the verifying-key bytes, the 38 fixed
+      columns' values and the 32 permutation columns' values (as the cell c * n + r of delta^c * omega^r); every other section (l0, l_last, l_active_row, polys, cosets)
+      is recomputed from them, and the manifest records the sha256 of the whole pk.key so a test can rebuild it byte for byte
   tests/golden/pk_k6_subset.npz     a few columns of the proving key:
       fixed_values/fixed_polys/fixed_cosets[c]  c in FIXED_COLS, perm_{values,polys,cosets}[0],
       l0, l_last, l_active_row   -- all as uint64[.,4] little-endian Montgomery limbs (the wire form)
-  tests/golden/manifest.json        sizes + sha256 of both, and the relations verified while generating
+  tests/golden/manifest.json        sizes + sha256 of every output and of pk.key, and the relations verified while generating
 
 Known-answer content these fixtures give the hot path:
   * 64 MSM known answers:  g_lagrange[j] = n^-1 * sum_i omega^(-ij) * g[i]     (pins MSM, omega, G1 add)
@@ -32,7 +36,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
 from oracle import pyref as ref  # noqa: E402
 
-ASSETS = "/root/reference/tests/assets"
+ASSETS = os.environ.get("EZKL_ASSETS", "ezkl/tests/assets")
 FIXED_COLS = [0, 1, 5, 37]
 
 
@@ -100,6 +104,26 @@ def frs(b: bytes):
     return [ref.fr_from_wire(b[i:i + 32]) for i in range(0, len(b), 32)]
 
 
+def frs_mont(b: bytes):
+    return [int.from_bytes(b[i:i + 32], "little") for i in range(0, len(b), 32)]
+
+
+def write_primary_and_proof():
+    d = open(os.path.join(ASSETS, "pk.key"), "rb").read()
+    pk = parse_pk(d)
+    vk_len = 7 + 64 * 38 + 64 * 32 + 80 * ((1 << pk["k"]) // 8)
+    # a permutation column's values are delta^c * omega^r (the cell (c, r) its cycle maps to): stored as c * n + r
+    n = 1 << pk["k"]
+    delta, w = pow(7, 1 << 28, ref.R), ref.omega_for(pk["k"])
+    cell = {ref.to_mont(pow(delta, c, ref.R) * pow(w, r, ref.R) % ref.R, ref.R): c * n + r for c in range(len(pk["perms"])) for r in range(n)}
+    cells = np.array([[cell[x] for x in frs_mont(col)] for col in pk["perms"]], np.uint16)
+    np.savez_compressed(os.path.join(HERE, "pk_k6_primary.npz"), vk=np.frombuffer(d[:vk_len], np.uint8),
+                        fixed_values=np.stack([limbs(c) for c in pk["fixed_values"]]), permutation_cells=cells)
+    proof = bytes(json.load(open(os.path.join(ASSETS, "proof.json")))["proof"])
+    with open(os.path.join(HERE, "reference_proof_k6.bin"), "wb") as f:
+        f.write(proof)
+
+
 def main():
     checks = []
     srs = open(os.path.join(ASSETS, "kzg"), "rb").read()
@@ -147,9 +171,12 @@ def main():
     checks.append("pk: l0 == coset-extended L_0, l_last == coset-extended L_{n-6}")
     out["l0"], out["l_last"], out["l_active_row"] = limbs(pk["l0"]), limbs(pk["l_last"]), limbs(pk["l_active_row"])
     np.savez_compressed(os.path.join(HERE, "pk_k6_subset.npz"), **out)
+    write_primary_and_proof()
 
     man = {"source": "zkonduit/ezkl tests/assets/{kzg,pk.key}", "k": 6, "ext_k": ext_k, "checks": checks}
-    for fn in ("kzg_k6.srs", "pk_k6_subset.npz"):
+    pk_key = open(os.path.join(ASSETS, "pk.key"), "rb").read()
+    man["pk.key"] = {"bytes": len(pk_key), "sha256": hashlib.sha256(pk_key).hexdigest()}
+    for fn in ("kzg_k6.srs", "pk_k6_subset.npz", "pk_k6_primary.npz", "reference_proof_k6.bin"):
         b = open(os.path.join(HERE, fn), "rb").read()
         man[fn] = {"bytes": len(b), "sha256": hashlib.sha256(b).hexdigest()}
     json.dump(man, open(os.path.join(HERE, "manifest.json"), "w"), indent=1)

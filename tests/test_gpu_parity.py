@@ -1,6 +1,6 @@
 """GPU parity tests: the CUDA path (through the C ABI / the halo2-mirror host layer) against the CPU oracle, the
 reference's golden fixtures, and size-independent properties at BASELINE.json's full sizes.  Bit-exact everywhere
-(integer arithmetic); run on the B200 box with `pytest -m gpu`."""
+(integer arithmetic); run on an H100 with `pytest -m gpu`."""
 import ctypes as C
 import random
 

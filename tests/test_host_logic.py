@@ -118,11 +118,38 @@ def test_signed_window_recoding(c):
         assert all(-(1 << (c - 1)) <= int(d) <= (1 << (c - 1)) for d in out[i])
 
 
-def test_proving_key_reader_on_reference_fixture():
-    """ProvingKey::read mirror against the reference's own tests/assets/pk.key (present in the build container only)."""
-    path = "/root/reference/tests/assets/pk.key"
-    if not os.path.exists(path):
-        pytest.skip("reference checkout not present (GPU box)")
+def reference_pk_key(monkeypatch, path):
+    """Rebuilds the reference's own tests/assets/pk.key at `path`, byte for byte (its sha256 is in tests/golden/manifest.json):
+    the sections keygen does not derive come from tests/golden/pk_k6_primary.npz, the others are recomputed on the CPU backend
+    and laid out as ProvingKey::write (RawBytes) does: a poly is a u32 BE length and its limbs, a slice of polys is a u32 BE
+    count and a u32 BE length per poly, then the polys."""
+    import hashlib
+    import json
+    import struct
+    from ezkl_b200 import halo2 as h2
+    from tests import cpu_backend as cb
+    cb.patch_backend(monkeypatch)
+    prim = np.load(os.path.join(H.GOLDEN, "pk_k6_primary.npz"))
+    key = h2.ProvingKey()
+    key.k = 6
+    delta, w = pow(7, 1 << 28, pyref.R), pyref.omega_for(6)           # permutation values are delta^c * omega^r, stored as c * 64 + r
+    key.fixed_values = list(prim["fixed_values"])
+    key.permutations = [np.stack([H.fr_wire(pow(delta, int(x) >> 6, pyref.R) * pow(w, int(x) & 63, pyref.R)) for x in col]) for col in prim["permutation_cells"]]
+    der = key.keygen_pk_polys(9, 5)
+    poly = lambda p: struct.pack(">I", len(p)) + np.ascontiguousarray(p, np.uint64).tobytes()
+    slc = lambda ps: struct.pack(">I", len(ps)) + struct.pack(">%dI" % len(ps), *[len(p) for p in ps]) + b"".join(poly(p) for p in ps)
+    data = (prim["vk"].tobytes() + poly(der["l0"]) + poly(der["l_last"]) + poly(der["l_active_row"]) + slc(key.fixed_values)
+            + slc(der["fixed_polys"]) + slc(der["fixed_cosets"]) + slc(key.permutations) + slc(der["permutation_polys"]) + slc(der["permutation_cosets"]))
+    assert hashlib.sha256(data).hexdigest() == json.load(open(os.path.join(H.GOLDEN, "manifest.json")))["pk.key"]["sha256"]
+    with open(path, "wb") as f:
+        f.write(data)
+    monkeypatch.undo()
+    return path
+
+
+def test_proving_key_reader_on_reference_fixture(monkeypatch, tmp_path):
+    """ProvingKey::read mirror against the reference's own tests/assets/pk.key."""
+    path = reference_pk_key(monkeypatch, str(tmp_path / "pk.key"))
     from ezkl_b200 import halo2 as h2
     pk = h2.ProvingKey.read(path, num_permutation_columns=32, num_selectors=80)
     g = H.load_pk_fixture()

@@ -71,12 +71,12 @@ def test_transcript_rules():
 
 
 def test_reference_proof_fixture_parses_with_the_read_transcript():
-    """The reference's own proof fixture (/root/reference/tests/assets/proof.json, made by the Rust prover): 114 commitments,
-    231 evaluations, 2 SHPLONK points — every point must pass the on-curve check of EvmTranscriptRead, every scalar must be canonical."""
-    path = "/root/reference/tests/assets/proof.json"
-    if not os.path.exists(path):
-        pytest.skip("reference checkout not present (GPU box)")
-    proof = bytes(json.load(open(path))["proof"])
+    """The reference's own proof fixture (the `proof` bytes of ezkl's tests/assets/proof.json, made by the Rust prover, stored as
+    tests/golden/reference_proof_k6.bin): 114 commitments, 231 evaluations, 2 SHPLONK points — every point must pass the on-curve
+    check of EvmTranscriptRead, every scalar must be canonical."""
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_proof_k6.bin")
+    proof = open(path, "rb").read()
+    assert hashlib.sha256(proof).hexdigest() == json.load(open(os.path.join(os.path.dirname(path), "manifest.json")))["reference_proof_k6.bin"]["sha256"]
     rd = ts.EvmTranscriptRead(proof)
     assert len(proof) == 114 * 64 + 231 * 32 + 2 * 64
     pts = [rd.read_ec_point() for _ in range(114)]

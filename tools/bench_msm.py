@@ -8,6 +8,7 @@ import torch  # noqa: E402
 
 from ezkl_b200 import _native as nat  # noqa: E402
 from ezkl_b200 import device as dev  # noqa: E402
+import gpu_peaks  # noqa: E402
 
 
 def run(bases, sc, reps=3):
@@ -25,6 +26,8 @@ def run(bases, sc, reps=3):
 def sweep():
     """BASELINE configs[3]: standalone MSM sweep 2^16 .. 2^26 on one GPU (default window), batch 1 and 4."""
     import json
+    peak, peak_src = gpu_peaks.hbm_peak_gbs()
+    print("# hbm_frac against %.0f GB/s (%s)" % (peak, peak_src), flush=True)
     res = []
     for k in range(16, 27, 2):
         n = 1 << k
@@ -37,7 +40,7 @@ def sweep():
                 continue
             sc = dev.random_scalars(n, batch=batch, seed=5)
             ms = run(bases, sc, reps=2 if k >= 24 else 3)
-            res.append({"k": k, "batch": batch, "ms": round(ms, 3), "pairs_per_s": round(batch * n / ms * 1e3, 1), "hbm_frac": round(batch * n * (32 + 64 / batch) / (ms * 1e-3) / 6486.1e9, 5)})
+            res.append({"k": k, "batch": batch, "ms": round(ms, 3), "pairs_per_s": round(batch * n / ms * 1e3, 1), "hbm_frac": round(batch * n * (32 + 64 / batch) / (ms * 1e-3) / (peak * 1e9), 5)})
             print(res[-1], flush=True)
             del sc
         bases.release()

@@ -1,9 +1,8 @@
 #!/usr/bin/env python
-"""Column-polynomial kernels against the HBM roofline (run on the GPU box): the only genuinely bandwidth-bound kernels on the path.
+"""Column-polynomial kernels against the HBM roofline (run on an H100): the only genuinely bandwidth-bound kernels on the path.
 For each op and size, CUDA-event time over buffers larger than L2 (batch of columns back to back), algorithmic bytes per element
 (BASELINE.md §3: add/sub/mul/axpy 96 B, scale / scale_cycle / batch_invert 64 B, eval 32 B, scans / kate_division 64 B) and the
 fraction of the measured copy bandwidth (MEASURED_PEAKS.json)."""
-import json
 import os
 import sys
 
@@ -14,6 +13,7 @@ import torch  # noqa: E402
 from ezkl_b200 import _native as nat  # noqa: E402
 from ezkl_b200 import device as dev  # noqa: E402
 from ezkl_b200 import fields as F  # noqa: E402
+import gpu_peaks  # noqa: E402
 
 
 def timeit(fn, reps=10):
@@ -31,14 +31,10 @@ def timeit(fn, reps=10):
 
 def main():
     nat.init(0)
-    peak = 6486.1
-    try:
-        peak = float(json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"])
-    except Exception:
-        pass
+    peak, peak_src = gpu_peaks.hbm_peak_gbs()
     one = F.fr_to_limbs(1)
     s = F.fr_to_limbs(0x1234567)
-    print("# op, log2(n), columns, ms, G elts/s, algorithmic GB/s, fraction of measured HBM peak (%.0f GB/s)" % peak)
+    print("# op, log2(n), columns, ms, G elts/s, algorithmic GB/s, fraction of the HBM peak (%.0f GB/s, %s)" % (peak, peak_src))
     for k, batch in ((17, 96), (20, 12), (22, 3)):
         n = 1 << k
         a = dev.random_scalars(n, batch=batch, seed=1)

@@ -1,10 +1,9 @@
 // fd.cuh — BN254 Fr / Fq Montgomery arithmetic on 5 x 52-bit limbs with the limb products formed on the FP64 pipe.
 //
-// Why a second multiplier: every hot kernel of this library is bound by ONE pipe — ncu shows sm__pipe_fmaheavy_cycles_active
-// at ~90 % (IMAD.WIDE lives there) while the FP64 pipe sits at 0 %, the ALU pipe at ~30 % and 60 % of the issue slots are idle
-// (profiles/r02_ncu_pipe_breakdown.txt).  B200 keeps a full-rate FP64 pipe (64 DFMA/clk/SM nominal, 52.9 measured,
-// profiles/r01_pipe_probes.txt), so a multiplier whose product array runs on DFMA can execute NEXT TO the integer one
-// (different warps of the same kernel) and raise the SM's multiply throughput above what either pipe gives alone.
+// Why a second multiplier: every hot kernel of this library is bound by ONE pipe, the one IMAD / IMAD.WIDE issue on, while the
+// FP64 pipe has nothing to do (not measured on the H100).  The H100 SXM keeps a full-rate FP64 pipe (64 DFMA/clk/SM nominal), so a
+// multiplier whose product array runs on DFMA can execute NEXT TO the integer one (different warps of the same kernel) and raise
+// the SM's multiply throughput above what either pipe gives alone.
 //
 // Representation: Fd = 5 limbs of 52 bits held in uint64 (the integer 0 <= v < 2^260), Montgomery radix R' = 2^260.
 // A limb product a_j * b_i < 2^104 is split exactly with two fused multiply-adds in round-toward-zero mode

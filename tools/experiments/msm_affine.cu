@@ -1,7 +1,7 @@
 // msm_affine.cu — EXPERIMENT, not part of libezkl_b200.so: kernels and orchestration of the fused batched-affine bucket accumulation
 // (see msm_affine.cuh).  Per MSM call: one producer pass, then per round one fused consumer/producer kernel and one small inversion
-// kernel, then the hand-over to the XYZZ combine / reduce tail.  Wired into msm_run at commit e30e8c9 it is bit-exact and 2.1x slower
-// than the XYZZ chain (profiles/r02_msm_affine_fused_vs_xyzz.txt); the host bodies stay under test through the debug library.
+// kernel, then the hand-over to the XYZZ combine / reduce tail.  Wired into msm_run at commit e30e8c9 it is bit-exact and was measured
+// slower than the XYZZ chain; the host bodies stay under test through the debug library.
 #include <vector>
 #include "../../ezkl_b200/csrc/msm.cuh"
 #include "msm_affine.cuh"

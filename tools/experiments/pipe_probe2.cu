@@ -1,4 +1,4 @@
-// pipe_probe2.cu — what does a carry cost on the integer-multiply pipe of sm_100a?  (standalone: nvcc -o pipe_probe2 pipe_probe2.cu)
+// pipe_probe2.cu — what does a carry cost on the integer-multiply pipe of sm_90a?  (standalone: nvcc -o pipe_probe2 pipe_probe2.cu)
 // Every variant keeps 8 independent 64-bit accumulators per thread in aligned register pairs (declared as 64-bit operands and split
 // inside the asm block, so ptxas needs no repacking moves) and issues 8 multiply-accumulates per loop iteration:
 //   A  mad.wide.u32                                   -> IMAD.WIDE.U32             (no carry at all)
@@ -67,9 +67,10 @@ __global__ void __launch_bounds__(256) k_probe(uint64_t* out, int iters) {
 
 template <int V>
 static void run(const char* name, int per_iter_mul, int per_iter_add) {
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
-    int clock_khz = 1965000;
+    int clock_khz = 1980000;
+    cudaDeviceGetAttribute(&clock_khz, cudaDevAttrClockRate, 0);
     for (int bps = 2; bps <= 8; bps *= 2) {
         const int blocks = sms * bps, threads = 256, iters = 4000;
         uint64_t* d; cudaMalloc(&d, 8ull * blocks * threads);

@@ -10,6 +10,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ezkl_b200 import _native as nat  # noqa: E402
+import gpu_peaks  # noqa: E402
 
 P = 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47
 R = 0x30644e72e131a029b85045b68181585d2833e84879b9709143e1f593f0000001
@@ -38,7 +39,7 @@ def main():
         print("fd_mul on device, field %d: %d cases, %d mismatches" % (fid, len(xs), bad), flush=True)
     for threads, bps in ((256, 2), (256, 4), (256, 8)):
         for r in range(9):
-            iters, blocks = 2000, 148 * bps
+            iters, blocks = 2000, gpu_peaks.sm_count() * bps
             ms = C.c_float(0)
             nat.check(D.b200_debug_bench(10 + r, iters, blocks, threads, C.byref(ms)))
             ops = blocks * threads * iters

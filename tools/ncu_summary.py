@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise `ncu --set full` reports (read here, no GPU needed): per captured launch the duration, DRAM bytes, the pipe
 utilisation that names the saturated pipe, issue activity, occupancy and the warp-stall breakdown.
-usage: python tools/ncu_summary.py rep1.ncu-rep [rep2.ncu-rep ...] > profiles/rNN_xxx.txt"""
+usage: python tools/ncu_summary.py rep1.ncu-rep [rep2.ncu-rep ...] > summary.txt"""
 import csv
 import io
 import re

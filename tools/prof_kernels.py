@@ -13,6 +13,7 @@ from ezkl_b200 import _native as nat  # noqa: E402
 from ezkl_b200 import device as dev  # noqa: E402
 from ezkl_b200 import fields as F  # noqa: E402
 from ezkl_b200 import halo2 as h2  # noqa: E402
+import gpu_peaks  # noqa: E402
 
 
 def microbench():
@@ -23,7 +24,7 @@ def microbench():
             if variant == 3 and threads * blocks_per_sm > 512:
                 continue
             iters = 2000 if variant != 3 else 200
-            blocks = 148 * blocks_per_sm
+            blocks = gpu_peaks.sm_count() * blocks_per_sm
             ms = C.c_float(0)
             nat.check(nat.dbg_lib().b200_debug_bench(variant, iters, blocks, threads, C.byref(ms)))
             ops = blocks * threads * iters
@@ -33,15 +34,16 @@ def microbench():
 def pipebench():
     L = nat.lib()
     names = {0: "mad.wide.u32 (IMAD.WIDE, no carry)", 1: "mad.lo.cc/madc.hi.cc pairs (IMAD.WIDE.X)", 2: "mad.lo.u32 (IMAD)", 3: "fma.f64 (DFMA)"}
+    sms, clock_hz = gpu_peaks.sm_count(), gpu_peaks.max_sm_clock_hz()
     for variant in (0, 1, 2, 3):
         for threads, bps in ((256, 2), (256, 4), (256, 8)):
-            iters, blocks = 4000, 148 * bps
+            iters, blocks = 4000, sms * bps
             ms = C.c_float(0)
             nat.check(nat.dbg_lib().b200_debug_bench_pipe(variant, iters, blocks, threads, C.byref(ms)))
             per_iter = 16 if variant == 1 else 8          # PTX ops per thread per iteration (v1: 8 lo/hi pairs = 8 fused wide ops)
             ops = blocks * threads * iters * per_iter
-            clk = ms.value * 1e-3 * 1.965e9
-            print("%-44s threads/SM=%5d  %8.3f ms  %8.1f PTX-ops/clk/SM  (%6.2f T ops/s)" % (names[variant], threads * bps, ms.value, ops / clk / 148, ops / ms.value / 1e9), flush=True)
+            clk = ms.value * 1e-3 * clock_hz         # at the maximum SM clock: a power-capped card that runs slower shows fewer ops / clk
+            print("%-44s threads/SM=%5d  %8.3f ms  %8.1f PTX-ops/clk/SM  (%6.2f T ops/s)" % (names[variant], threads * bps, ms.value, ops / clk / sms, ops / ms.value / 1e9), flush=True)
 
 
 def workload(k, batch, c):
