@@ -60,7 +60,6 @@ static std::atomic<int> g_ndev{0};
 static std::atomic<bool> g_inited{false};
 static std::atomic<int> g_active{0};            // entry points in flight (b200_shutdown waits for them)
 static std::atomic<uint64_t> g_epoch{1};        // bumped by b200_shutdown: contexts of an older epoch are gone
-static std::atomic<uint64_t> g_launches{0};
 static std::mutex g_mu;                         // tables, plans, context registry
 
 // One registered base vector: a window-precomputed table replica per device of the process.
@@ -191,8 +190,12 @@ static inline Fr as_fr(const b200_fr* p) { Fr r; memcpy(&r, p, sizeof r); return
 // ---- large host <-> device copies of PAGEABLE caller memory (what a Rust Vec<Fr> is) ------------------------------------------------
 // cudaMemcpyAsync from pageable memory is limited by one driver thread copying into its own staging buffer.  Here the
 // copy is cut into 16 MiB chunks that four host threads move into a pinned bounce buffer while the DMA engine drains the other one, so
-// the PCIe link (Gen5 x16) is fed at memcpy-pool speed.  Small copies keep the plain path.
+// the PCIe link (Gen5 x16) is fed at memcpy-pool speed.  Copies below DIRECT_MAX_BYTES keep the plain path.  Measured with a host-pointer
+// poly_op on fresh numpy buffers (two uploads and one download of S MiB) on an H100 80GB HBM3 at a 700 W power limit, median ms of
+// two runs, plain vs bounce: S = 8: 1.7 / 1.6 vs 2.9 / 3.7;  16: 3.4 / 4.0 vs 4.6 / 4.6;  20: 5.5 / 5.2 vs 5.6 / 5.3;
+// 24: 9.0 / 6.0 vs 5.8 / 6.1;  28: 10.1 / 8.1 vs 6.3 / 6.2;  32: 21.3 / 20.8 vs 13.0 / 11.9.  The crossover is at about 24 MiB.
 static constexpr size_t BOUNCE_BYTES = (size_t)16 << 20;
+static constexpr size_t DIRECT_MAX_BYTES = (size_t)24 << 20;
 struct HostSeg { uint8_t* p; size_t bytes; };          // one caller buffer (a column); a list of them maps onto ONE contiguous device range
 // copies bytes [lo, hi) of the virtual concatenation of `segs` between the caller's buffers and `flat` (the pinned slot, offset 0 = byte lo0)
 static void seg_copy_range(const HostSeg* segs, size_t nsegs, size_t lo0, size_t lo, size_t hi, uint8_t* flat, bool to_flat) {
@@ -231,7 +234,7 @@ static int bounce_ready(Ctx* c) {
 static int h2d_segments(Ctx* c, void* d_dst, const HostSeg* segs, size_t nsegs, cudaStream_t st) {
     size_t total = 0;
     for (size_t i = 0; i < nsegs; ++i) total += segs[i].bytes;
-    if (total < ((size_t)8 << 20)) {
+    if (total < DIRECT_MAX_BYTES) {
         size_t off = 0;
         for (size_t i = 0; i < nsegs; ++i) { B200_CUDA(cudaMemcpyAsync((uint8_t*)d_dst + off, segs[i].p, segs[i].bytes, cudaMemcpyHostToDevice, st)); off += segs[i].bytes; }
         return 0;
@@ -251,7 +254,7 @@ static int h2d_segments(Ctx* c, void* d_dst, const HostSeg* segs, size_t nsegs, 
 static int d2h_segments(Ctx* c, const void* d_src, const HostSeg* segs, size_t nsegs, cudaStream_t st) {
     size_t total = 0;
     for (size_t i = 0; i < nsegs; ++i) total += segs[i].bytes;
-    if (total < ((size_t)8 << 20)) {
+    if (total < DIRECT_MAX_BYTES) {
         size_t off = 0;
         for (size_t i = 0; i < nsegs; ++i) { B200_CUDA(cudaMemcpyAsync(segs[i].p, (const uint8_t*)d_src + off, segs[i].bytes, cudaMemcpyDeviceToHost, st)); off += segs[i].bytes; }
         B200_CUDA(cudaStreamSynchronize(st));
@@ -341,14 +344,24 @@ static NttPlan* warm_plan(int slot, uint32_t log_n, const Fr& omega, cudaStream_
     return p;
 }
 
-static int ntt_call(Ctx* c, const Fr* src, size_t src_stride, size_t n_in, Fr* tmp, Fr* dst, size_t dst_stride, uint32_t log_n,
-                    const Fr& omega, const NttScale& pre, const NttScale& post, int batch, cudaStream_t st) {
+// ---- internal call layer: <op>_on(c, st, ...) validates the device-side arguments, converts host constants and runs the
+//      kernel file's *_run on `st`.  A _dev entry point is B200_ENTER + StreamScope + <op>_on; a host-pointer entry point stages
+//      the caller's buffers in and out around the same <op>_on, inside one StreamScope on the thread's library stream.
+static int ntt_call(Ctx* c, cudaStream_t st, const Fr* src, size_t src_stride, size_t n_in, Fr* tmp, Fr* dst, size_t dst_stride, uint32_t log_n,
+                    const Fr& omega, const NttScale& pre, const NttScale& post, int batch) {
     if (log_n < 1 || log_n > 28) { set_error("ntt: log_n = %u out of range [1, 28]", log_n); return -1; }
     NttPlan* plan = warm_plan(c->slot, log_n, omega, st);         // looked up / built under g_mu; the vector of plans is never touched unlocked
     if (!plan) return -2;
-    int rc = ntt_run(plan, src, src_stride, n_in, tmp, (size_t)1 << log_n, dst, dst_stride, log_n, omega, pre, post, batch, st);
-    if (!rc) g_launches += (uint64_t)ntt_launches_per_run(log_n);
-    return rc;
+    return ntt_run(plan, src, src_stride, n_in, tmp, (size_t)1 << log_n, dst, dst_stride, log_n, omega, pre, post, batch, st);
+}
+// the (mode, constants) pairs of the C ABI -> NttScale
+static int ntt_scales(int pre_mode, const b200_fr* pre, int post_mode, const b200_fr* post, NttScale* a, NttScale* b) {
+    B200_CHECK((pre_mode == 0 || pre_mode == 1 || pre_mode == 3) && (post_mode == 0 || post_mode == 1 || post_mode == 3), -1, "ntt: scale mode must be 0, 1 or 3");
+    B200_CHECK((pre_mode == 0 || pre) && (post_mode == 0 || post), -1, "ntt: scale constants missing");
+    a->mode = pre_mode; b->mode = post_mode;
+    for (int i = 0; i < pre_mode; ++i) a->c[i] = as_fr(pre + i);
+    for (int i = 0; i < post_mode; ++i) b->c[i] = as_fr(post + i);
+    return 0;
 }
 
 // ---- device workers: one host thread per extra device, so that the host-pointer entry points of a multi-device process drive
@@ -399,7 +412,7 @@ static int run_on_slots(int nslots, const std::function<int(int)>& fn) {
 
 // ---- MSM building blocks ------------------------------------------------------------------------------------------------------
 // device-resident columns on the context's device -> XYZZ partial sums on that device (sub-batches bounded by the scratch budget)
-static int msm_dev_on(Ctx* c, const BaseSet* bs, const Fr* sc, size_t n, size_t stride, size_t batch, size_t base_off, G1Xyzz* out, cudaStream_t st) {
+static int msm_dev_on(Ctx* c, cudaStream_t st, const BaseSet* bs, const Fr* sc, size_t n, size_t stride, size_t batch, size_t base_off, G1Xyzz* out) {
     const MsmTable* t = bs->t[c->slot];
     B200_CHECK(t, -1, "msm: the bases have no replica on device slot %d", c->slot);
     const size_t per_col = msm_workspace_per_column(*t, n);
@@ -409,7 +422,6 @@ static int msm_dev_on(Ctx* c, const BaseSet* bs, const Fr* sc, size_t n, size_t 
     for (size_t b0 = 0; b0 < batch; b0 += sub) {
         const size_t nb = batch - b0 < sub ? batch - b0 : sub;
         if (int rc = msm_run(*t, sc + b0 * stride, n, stride, (int)nb, out + b0, c->msm_ws, st, base_off)) return rc;
-        g_launches += (uint64_t)msm_launches_per_run();
     }
     return 0;
 }
@@ -431,7 +443,7 @@ static int msm_host_on(Ctx* c, const BaseSet* bs, const b200_fr* const* cols, si
             segs[b] = HostSeg{(uint8_t*)const_cast<b200_fr*>(cols[b0 + b] + base_off), sizeof(Fr) * n};
         }
         if (int rc = h2d_segments(c, c->stage_a.p, segs.data(), nb, ss.st)) return rc;
-        if (int rc = msm_dev_on(c, bs, c->stage_a.as<Fr>(), n, n, nb, base_off, c->small.as<G1Xyzz>() + b0, ss.st)) return rc;
+        if (int rc = msm_dev_on(c, ss.st, bs, c->stage_a.as<Fr>(), n, n, nb, base_off, c->small.as<G1Xyzz>() + b0)) return rc;
         if (b0 + nb < count) B200_CUDA(cudaStreamSynchronize(ss.st));      // the staging buffer is reused by the next sub-batch
     }
     B200_CUDA(cudaMemcpyAsync(h_out, c->small.p, sizeof(G1Xyzz) * count, cudaMemcpyDeviceToHost, ss.st));
@@ -588,8 +600,7 @@ int b200_sync_all(void) {
 }
 
 // ---- bases ---------------------------------------------------------------------------------------------------
-int b200_bases_register_dev(const void* d_bases, size_t n, int window_bits, uint64_t* handle) {
-    B200_ENTER(c, d_bases);
+static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, size_t n, int window_bits, uint64_t* handle) {
     B200_CHECK(d_bases && handle && n > 0, -1, "bases_register: null argument or n == 0");
     B200_CHECK(window_bits == 0 || (window_bits >= 4 && window_bits <= 24), -1, "bases_register: window_bits %d not in {0, 4..24}", window_bits);
     BaseSet* bs = new BaseSet();
@@ -601,8 +612,7 @@ int b200_bases_register_dev(const void* d_bases, size_t n, int window_bits, uint
     };
     MsmTable* t = new MsmTable();
     bs->t[c->slot] = t;
-    if (int rc = msm_table_build(t, reinterpret_cast<const G1Affine*>(d_bases), n, window_bits, c->stream)) return fail(rc);
-    g_launches += (uint64_t)(t->W - 1);
+    if (int rc = msm_table_build(t, reinterpret_cast<const G1Affine*>(d_bases), n, window_bits, st)) return fail(rc);
     bs->n = n; bs->c = t->c; bs->W = t->W;
     // replicas: the finished table crosses NVLink once per extra device (cheaper than rebuilding: one inversion per point and level)
     for (int s = 0; s < g_ndev.load(); ++s) if (s != c->slot) {
@@ -613,22 +623,27 @@ int b200_bases_register_dev(const void* d_bases, size_t n, int window_bits, uint
         cudaError_t e = cudaMalloc(&r->d_table, sizeof(G1Affine) * n * t->W);
         cudaSetDevice(c->dev);
         if (e != cudaSuccess) { set_error("bases_register: replica on device %d: %s", r->device, cudaGetErrorString(e)); return fail(-2); }
-        e = cudaMemcpyPeerAsync(r->d_table, r->device, t->d_table, t->device, sizeof(G1Affine) * n * t->W, c->stream);
+        e = cudaMemcpyPeerAsync(r->d_table, r->device, t->d_table, t->device, sizeof(G1Affine) * n * t->W, st);
         if (e != cudaSuccess) { set_error("bases_register: peer copy: %s", cudaGetErrorString(e)); return fail(-2); }
     }
-    cudaError_t e = cudaStreamSynchronize(c->stream);
+    cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("bases_register: %s", cudaGetErrorString(e)); return fail(-2); }
     std::lock_guard<std::mutex> lk(g_mu);
     *handle = g_next_handle++;
     g_tables[*handle] = bs;
     return 0;
 }
+int b200_bases_register_dev(const void* d_bases, size_t n, int window_bits, uint64_t* handle) {
+    B200_ENTER(c, d_bases); StreamScope ss(c, nullptr);
+    return bases_register_on(c, ss.st, d_bases, n, window_bits, handle);
+}
 int b200_bases_register(const b200_g1_affine* bases, size_t n, int window_bits, uint64_t* handle) {
     B200_ENTER(c, nullptr);
     B200_CHECK(bases && handle && n > 0, -1, "bases_register: null argument or n == 0");
     if (c->stage_a.ensure(sizeof(G1Affine) * n)) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, bases, sizeof(G1Affine) * n, cudaMemcpyHostToDevice, c->stream));
-    return b200_bases_register_dev(c->stage_a.p, n, window_bits, handle);
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_one(c, c->stage_a.p, bases, sizeof(G1Affine) * n, ss.st)) return rc;
+    return bases_register_on(c, ss.st, c->stage_a.p, n, window_bits, handle);
 }
 int b200_bases_release(uint64_t handle) {
     CallGuard cg; if (!cg.ok) return -3;
@@ -665,7 +680,7 @@ int b200_msm_batch_dev(uint64_t bases, const void* d_scalars, size_t n, size_t s
     B200_CHECK(batch <= 1 || stride >= n, -1, "msm: column stride %zu < column length %zu", stride, n);
     if (batch == 0) return 0;
     StreamScope ss(c, stream);
-    return msm_dev_on(c, t, reinterpret_cast<const Fr*>(d_scalars), n, stride, batch, 0, reinterpret_cast<G1Xyzz*>(d_out_xyzz), ss.st);
+    return msm_dev_on(c, ss.st, t, reinterpret_cast<const Fr*>(d_scalars), n, stride, batch, 0, reinterpret_cast<G1Xyzz*>(d_out_xyzz));
 }
 int b200_msm_batch(uint64_t bases, const b200_fr* const* scalars, size_t n, size_t batch, b200_g1_jac* out) {
     B200_ENTER(c, nullptr);
@@ -733,7 +748,7 @@ int b200_msm_sharded_dev(uint64_t bases, const void* const* d_scalar_slices, siz
         StreamScope ss(cs[s], nullptr);
         G1Xyzz* part = gather + batch * nd;           // device 0: a staging row behind the gather matrix
         if (s != 0) { if (cs[s]->small.ensure(sizeof(G1Xyzz) * batch)) { cudaSetDevice(cur); return -2; } part = cs[s]->small.as<G1Xyzz>(); }
-        if (int rc = msm_dev_on(cs[s], t, reinterpret_cast<const Fr*>(d_scalar_slices[s]), hi - lo, hi - lo, batch, lo, part, ss.st)) { cudaSetDevice(cur); return rc; }
+        if (int rc = msm_dev_on(cs[s], ss.st, t, reinterpret_cast<const Fr*>(d_scalar_slices[s]), hi - lo, hi - lo, batch, lo, part)) { cudaSetDevice(cur); return rc; }
         // partial sums travel to device 0 over NVLink: column b of device s lands at gather[b * nd + s]
         B200_CUDA(cudaMemcpy2DAsync(gather + s, sizeof(G1Xyzz) * nd, part, sizeof(G1Xyzz), sizeof(G1Xyzz), batch, cudaMemcpyDefault, ss.st));
     }
@@ -744,7 +759,6 @@ int b200_msm_sharded_dev(uint64_t bases, const void* const* d_scalar_slices, siz
         StreamScope ss(cs[0], nullptr);
         G1Xyzz* sums = gather + batch * (nd + 1);
         if (int rc = g1_sum_run(gather, batch, nd, sums, ss.st)) { cudaSetDevice(cur); return rc; }
-        g_launches += 1;
         B200_CUDA(cudaMemcpyAsync(h.data(), sums, sizeof(G1Xyzz) * batch, cudaMemcpyDeviceToHost, ss.st));
         B200_CUDA(cudaStreamSynchronize(ss.st));
     }
@@ -756,48 +770,41 @@ int b200_g1_sum_dev(const void* d_points_xyzz, size_t groups, size_t count, void
     B200_ENTER(c, d_points_xyzz);
     B200_CHECK(d_points_xyzz && d_out_xyzz, -1, "g1_sum: null pointer");
     StreamScope ss(c, stream);
-    int rc = g1_sum_run(reinterpret_cast<const G1Xyzz*>(d_points_xyzz), groups, count, reinterpret_cast<G1Xyzz*>(d_out_xyzz), ss.st);
-    if (!rc) g_launches += 1;
-    return rc;
+    return g1_sum_run(reinterpret_cast<const G1Xyzz*>(d_points_xyzz), groups, count, reinterpret_cast<G1Xyzz*>(d_out_xyzz), ss.st);
 }
-int b200_g1_fft_dev(const void* d_in_affine, uint32_t log_n, const b200_fr* omega, const b200_fr* scale, void* d_out_affine, void* stream) {
-    B200_ENTER(c, d_in_affine);
+static int g1_fft_on(Ctx* c, cudaStream_t st, const void* d_in_affine, uint32_t log_n, const b200_fr* omega, const b200_fr* scale, void* d_out_affine) {
     B200_CHECK(d_in_affine && omega && d_out_affine, -1, "g1_fft: null pointer");
     const Fr w = as_fr(omega);
     Fr sc = fp_one<FrTag>();
     if (scale) sc = as_fr(scale);
-    StreamScope ss(c, stream);
-    int rc = g1_fft_run(reinterpret_cast<const G1Affine*>(d_in_affine), log_n, w, scale ? &sc : nullptr, reinterpret_cast<G1Affine*>(d_out_affine), c->msm_ws.misc, ss.st);
-    if (!rc) g_launches += (uint64_t)g1_fft_launches(log_n);
-    return rc;
+    return g1_fft_run(reinterpret_cast<const G1Affine*>(d_in_affine), log_n, w, scale ? &sc : nullptr, reinterpret_cast<G1Affine*>(d_out_affine), c->msm_ws.misc, st);
+}
+int b200_g1_fft_dev(const void* d_in_affine, uint32_t log_n, const b200_fr* omega, const b200_fr* scale, void* d_out_affine, void* stream) {
+    B200_ENTER(c, d_in_affine); StreamScope ss(c, stream);
+    return g1_fft_on(c, ss.st, d_in_affine, log_n, omega, scale, d_out_affine);
 }
 int b200_g1_fft(const b200_g1_affine* in, uint32_t log_n, const b200_fr* omega, const b200_fr* scale, b200_g1_affine* out) {
     B200_ENTER(c, nullptr);
     B200_CHECK(in && omega && out && log_n <= 26, -1, "g1_fft: bad argument");
     const size_t n = (size_t)1 << log_n;
     if (c->stage_a.ensure(sizeof(G1Affine) * n) || c->stage_b.ensure(sizeof(G1Affine) * n)) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, in, sizeof(G1Affine) * n, cudaMemcpyHostToDevice, c->stream));
-    if (int rc = b200_g1_fft_dev(c->stage_a.p, log_n, omega, scale, c->stage_b.p, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(out, c->stage_b.p, sizeof(G1Affine) * n, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_one(c, c->stage_a.p, in, sizeof(G1Affine) * n, ss.st)) return rc;
+    if (int rc = g1_fft_on(c, ss.st, c->stage_a.p, log_n, omega, scale, c->stage_b.p)) return rc;
+    return d2h_one(c, out, c->stage_b.p, sizeof(G1Affine) * n, ss.st);
 }
 int b200_g1_fixed_base_mul_dev(const void* d_scalars, size_t n, const b200_g1_affine* base, void* d_out_affine, void* stream) {
     B200_ENTER(c, d_scalars);
     B200_CHECK(d_scalars && base && d_out_affine, -1, "g1_fixed_base_mul: null pointer");
     G1Affine b; memcpy(&b, base, sizeof b);
     StreamScope ss(c, stream);
-    int rc = g1_fixed_base_mul_run(reinterpret_cast<const Fr*>(d_scalars), n, b, reinterpret_cast<G1Affine*>(d_out_affine), ss.st);
-    if (!rc && n) g_launches += 1;
-    return rc;
+    return g1_fixed_base_mul_run(reinterpret_cast<const Fr*>(d_scalars), n, b, reinterpret_cast<G1Affine*>(d_out_affine), ss.st);
 }
 int b200_g1_generate_dev(uint64_t seed, size_t n, void* d_out_affine, void* stream) {
     B200_ENTER(c, d_out_affine);
     B200_CHECK(d_out_affine, -1, "g1_generate: null pointer");
     StreamScope ss(c, stream);
-    int rc = g1_generate_run(seed, n, reinterpret_cast<G1Affine*>(d_out_affine), ss.st);
-    if (!rc && n) g_launches += 1;
-    return rc;
+    return g1_generate_run(seed, n, reinterpret_cast<G1Affine*>(d_out_affine), ss.st);
 }
 int b200_g1_normalize(const b200_g1_xyzz* points, size_t n, b200_g1_jac* out) {
     B200_CHECK(points && out, -1, "g1_normalize: null pointer");
@@ -813,16 +820,12 @@ int b200_ntt_dev(const void* d_src, size_t src_stride, size_t n_in, void* d_tmp,
                  const b200_fr* omega, int pre_mode, const b200_fr* pre, int post_mode, const b200_fr* post, size_t batch, void* stream) {
     B200_ENTER(c, d_src);
     B200_CHECK(d_src && d_tmp && d_dst && omega, -1, "ntt: null pointer");
-    B200_CHECK((pre_mode == 0 || pre_mode == 1 || pre_mode == 3) && (post_mode == 0 || post_mode == 1 || post_mode == 3), -1, "ntt: scale mode must be 0, 1 or 3");
-    B200_CHECK((pre_mode == 0 || pre) && (post_mode == 0 || post), -1, "ntt: scale constants missing");
-    if (batch == 0) return 0;
     NttScale a, b;
-    a.mode = pre_mode; b.mode = post_mode;
-    for (int i = 0; i < pre_mode; ++i) a.c[i] = as_fr(pre + i);
-    for (int i = 0; i < post_mode; ++i) b.c[i] = as_fr(post + i);
+    if (int rc = ntt_scales(pre_mode, pre, post_mode, post, &a, &b)) return rc;
+    if (batch == 0) return 0;
     StreamScope ss(c, stream);
-    return ntt_call(c, reinterpret_cast<const Fr*>(d_src), src_stride, n_in, reinterpret_cast<Fr*>(d_tmp), reinterpret_cast<Fr*>(d_dst), dst_stride,
-                    log_n, as_fr(omega), a, b, (int)batch, ss.st);
+    return ntt_call(c, ss.st, reinterpret_cast<const Fr*>(d_src), src_stride, n_in, reinterpret_cast<Fr*>(d_tmp), reinterpret_cast<Fr*>(d_dst), dst_stride,
+                    log_n, as_fr(omega), a, b, (int)batch);
 }
 
 // one transform of 2^log_n elements split across the devices of the process in contiguous natural-order slices (slice g of
@@ -843,7 +846,6 @@ static int ntt_sharded_on(Ctx* const* cs, int nd, const Fr* const* src, Fr* cons
     cudaSetDevice(cur);
     int rc = ntt_run_sharded(plans, nd, ids, src, tmp, dst, log_n, omega, pre, post, n_in, st, ev);
     for (int s = 0; s < nd && !rc; ++s) { cs[s]->last_stream = st[s]; cs[s]->has_last = true; }       // ev[s] was recorded after the last pass
-    if (!rc) g_launches += (uint64_t)ntt_launches_per_run(log_n) * nd;
     return rc;
 }
 int b200_ntt_sharded_dev(const void* const* d_src_slices, void* const* d_tmp_slices, void* const* d_dst_slices, uint32_t log_n, size_t n_in, const b200_fr* omega,
@@ -852,12 +854,8 @@ int b200_ntt_sharded_dev(const void* const* d_src_slices, void* const* d_tmp_sli
     const int nd = g_ndev.load();
     B200_CHECK(nd >= 2, -1, "ntt_sharded: needs a multi-device process (b200_init_multi)");
     B200_CHECK(d_src_slices && d_tmp_slices && d_dst_slices && omega, -1, "ntt_sharded: null pointer");
-    B200_CHECK((pre_mode == 0 || pre_mode == 1 || pre_mode == 3) && (post_mode == 0 || post_mode == 1 || post_mode == 3), -1, "ntt: scale mode must be 0, 1 or 3");
-    B200_CHECK((pre_mode == 0 || pre) && (post_mode == 0 || post), -1, "ntt: scale constants missing");
     NttScale a, b;
-    a.mode = pre_mode; b.mode = post_mode;
-    for (int i = 0; i < pre_mode; ++i) a.c[i] = as_fr(pre + i);
-    for (int i = 0; i < post_mode; ++i) b.c[i] = as_fr(post + i);
+    if (int rc = ntt_scales(pre_mode, pre, post_mode, post, &a, &b)) return rc;
     Ctx* cs[MAX_DEV];
     for (int s = 0; s < nd; ++s) {
         if (int rc = get_ctx(&cs[s], s)) return rc;
@@ -887,7 +885,7 @@ static int ntt_host_on(Ctx* c, const b200_fr* const* src, b200_fr* const* dst, s
             down[p] = HostSeg{(uint8_t*)dst[b0 + p], sizeof(Fr) * N};
         }
         if (int rc = h2d_segments(c, c->stage_a.p, up.data(), nb, ss.st)) return rc;
-        if (int rc = ntt_call(c, c->stage_a.as<Fr>(), n_in, n_in, c->stage_b.as<Fr>(), c->stage_c.as<Fr>(), N, log_n, omega, pre, post, (int)nb, ss.st)) return rc;
+        if (int rc = ntt_call(c, ss.st, c->stage_a.as<Fr>(), n_in, n_in, c->stage_b.as<Fr>(), c->stage_c.as<Fr>(), N, log_n, omega, pre, post, (int)nb)) return rc;
         if (int rc = d2h_segments(c, c->stage_c.p, down.data(), nb, ss.st)) return rc;
     }
     return 0;
@@ -976,16 +974,16 @@ int b200_extended_to_coeff(b200_fr* a, uint32_t ext_k, const b200_fr* ext_omega_
 }
 
 // ---- polynomial ops --------------------------------------------------------------------------------------------
-int b200_poly_op_dev(int op, const void* d_a, const void* d_b, const b200_fr* s, void* d_out, size_t n, void* stream) {
-    B200_ENTER(c, d_a);
+static int poly_op_on(Ctx*, cudaStream_t st, int op, const void* d_a, const void* d_b, const b200_fr* s, void* d_out, size_t n) {
     B200_CHECK(op >= 0 && op <= 4, -1, "poly_op: unknown op %d", op);
     B200_CHECK(d_a && d_out && (op == POLY_SCALE || d_b) && (op < POLY_SCALE || s), -1, "poly_op: missing operand for op %d", op);
     Fr sv = fp_zero<FrTag>();
     if (s) sv = as_fr(s);
-    StreamScope ss(c, stream);
-    int rc = poly_binary(op, reinterpret_cast<const Fr*>(d_a), reinterpret_cast<const Fr*>(d_b), s ? &sv : nullptr, reinterpret_cast<Fr*>(d_out), n, ss.st);
-    if (!rc && n) g_launches += 1;
-    return rc;
+    return poly_binary(op, reinterpret_cast<const Fr*>(d_a), reinterpret_cast<const Fr*>(d_b), s ? &sv : nullptr, reinterpret_cast<Fr*>(d_out), n, st);
+}
+int b200_poly_op_dev(int op, const void* d_a, const void* d_b, const b200_fr* s, void* d_out, size_t n, void* stream) {
+    B200_ENTER(c, d_a); StreamScope ss(c, stream);
+    return poly_op_on(c, ss.st, op, d_a, d_b, s, d_out, n);
 }
 int b200_poly_op(int op, const b200_fr* a, const b200_fr* b, const b200_fr* s, b200_fr* out, size_t n) {
     B200_ENTER(c, nullptr);
@@ -994,22 +992,21 @@ int b200_poly_op(int op, const b200_fr* a, const b200_fr* b, const b200_fr* s, b
     const bool need_b = op != POLY_SCALE;
     B200_CHECK(!need_b || b, -1, "poly_op: missing operand b");
     if (c->stage_a.ensure(sizeof(Fr) * n) || (need_b && c->stage_b.ensure(sizeof(Fr) * n))) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, a, sizeof(Fr) * n, cudaMemcpyHostToDevice, c->stream));
-    if (need_b) B200_CUDA(cudaMemcpyAsync(c->stage_b.p, b, sizeof(Fr) * n, cudaMemcpyHostToDevice, c->stream));
-    if (int rc = b200_poly_op_dev(op, c->stage_a.p, need_b ? c->stage_b.p : nullptr, s, c->stage_a.p, n, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(out, c->stage_a.p, sizeof(Fr) * n, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_one(c, c->stage_a.p, a, sizeof(Fr) * n, ss.st)) return rc;
+    if (need_b) { if (int rc = h2d_one(c, c->stage_b.p, b, sizeof(Fr) * n, ss.st)) return rc; }
+    if (int rc = poly_op_on(c, ss.st, op, c->stage_a.p, need_b ? c->stage_b.p : nullptr, s, c->stage_a.p, n)) return rc;
+    return d2h_one(c, out, c->stage_a.p, sizeof(Fr) * n, ss.st);
 }
-int b200_poly_lincomb_dev(const void* const* d_polys, const b200_fr* scalars, size_t count, size_t n, void* d_out, void* stream) {
-    B200_ENTER(c, d_out);
+static int lincomb_on(Ctx* c, cudaStream_t st, const void* const* d_polys, const b200_fr* scalars, size_t count, size_t n, void* d_out) {
     B200_CHECK(d_out && (count == 0 || (d_polys && scalars)), -1, "poly_lincomb: null pointer");
     std::vector<Fr> sv(count);
     if (count) memcpy(sv.data(), scalars, sizeof(Fr) * count);
-    StreamScope ss(c, stream);
-    int rc = poly_lincomb(reinterpret_cast<const Fr* const*>(d_polys), sv.data(), count, reinterpret_cast<Fr*>(d_out), n, c->poly_ws, ss.st);
-    if (!rc && n) g_launches += 1;
-    return rc;
+    return poly_lincomb(reinterpret_cast<const Fr* const*>(d_polys), sv.data(), count, reinterpret_cast<Fr*>(d_out), n, c->poly_ws, st);
+}
+int b200_poly_lincomb_dev(const void* const* d_polys, const b200_fr* scalars, size_t count, size_t n, void* d_out, void* stream) {
+    B200_ENTER(c, d_out); StreamScope ss(c, stream);
+    return lincomb_on(c, ss.st, d_polys, scalars, count, n, d_out);
 }
 int b200_poly_lincomb(const b200_fr* const* polys, const b200_fr* scalars, size_t count, size_t n, b200_fr* out) {
     B200_ENTER(c, nullptr);
@@ -1023,48 +1020,45 @@ int b200_poly_lincomb(const b200_fr* const* polys, const b200_fr* scalars, size_
         ptrs[j] = c->stage_a.as<Fr>() + j * n;
         up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[j]), sizeof(Fr) * n};
     }
-    if (int rc = h2d_segments(c, c->stage_a.p, up.data(), count, c->stream)) return rc;
-    if (int rc = b200_poly_lincomb_dev(ptrs.data(), scalars, count, n, c->stage_b.p, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(out, c->stage_b.p, sizeof(Fr) * n, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_segments(c, c->stage_a.p, up.data(), count, ss.st)) return rc;
+    if (int rc = lincomb_on(c, ss.st, ptrs.data(), scalars, count, n, c->stage_b.p)) return rc;
+    return d2h_one(c, out, c->stage_b.p, sizeof(Fr) * n, ss.st);
 }
-int b200_poly_scale_cycle_dev(void* d_a, size_t n, const b200_fr* consts, uint32_t period, void* stream) {
-    B200_ENTER(c, d_a);
+static int scale_cycle_on(Ctx* c, cudaStream_t st, void* d_a, size_t n, const b200_fr* consts, uint32_t period) {
     B200_CHECK(d_a && consts && period > 0 && period <= 1024, -1, "poly_scale_cycle: bad argument");
-    StreamScope ss(c, stream);
-    cudaStream_t st = ss.st;
     const Fr* d_consts = reinterpret_cast<const Fr*>(c->ring.push(consts, sizeof(Fr) * period, st));
     if (!d_consts) {
         if (c->small.ensure(sizeof(Fr) * period)) return -2;
         B200_CUDA(cudaMemcpyAsync(c->small.p, consts, sizeof(Fr) * period, cudaMemcpyHostToDevice, st));
         d_consts = c->small.as<Fr>();
     }
-    int rc = poly_scale_cycle(reinterpret_cast<const Fr*>(d_a), d_consts, period, reinterpret_cast<Fr*>(d_a), n, st);
-    if (!rc && n) g_launches += 1;
-    return rc;
+    return poly_scale_cycle(reinterpret_cast<const Fr*>(d_a), d_consts, period, reinterpret_cast<Fr*>(d_a), n, st);
+}
+int b200_poly_scale_cycle_dev(void* d_a, size_t n, const b200_fr* consts, uint32_t period, void* stream) {
+    B200_ENTER(c, d_a); StreamScope ss(c, stream);
+    return scale_cycle_on(c, ss.st, d_a, n, consts, period);
 }
 int b200_poly_scale_cycle(b200_fr* a, size_t n, const b200_fr* consts, uint32_t period) {
     B200_ENTER(c, nullptr);
     B200_CHECK(a && consts, -1, "poly_scale_cycle: null pointer");
     if (n == 0) return 0;
     if (c->stage_a.ensure(sizeof(Fr) * n)) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, a, sizeof(Fr) * n, cudaMemcpyHostToDevice, c->stream));
-    if (int rc = b200_poly_scale_cycle_dev(c->stage_a.p, n, consts, period, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(a, c->stage_a.p, sizeof(Fr) * n, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_one(c, c->stage_a.p, a, sizeof(Fr) * n, ss.st)) return rc;
+    if (int rc = scale_cycle_on(c, ss.st, c->stage_a.p, n, consts, period)) return rc;
+    return d2h_one(c, a, c->stage_a.p, sizeof(Fr) * n, ss.st);
 }
-int b200_poly_eval_batch_dev(const void* d_polys, size_t stride, size_t n, const b200_fr* x, size_t batch, void* d_out, void* stream) {
-    B200_ENTER(c, d_polys);
+static int eval_batch_on(Ctx* c, cudaStream_t st, const void* d_polys, size_t stride, size_t n, const b200_fr* x, size_t batch, void* d_out) {
     B200_CHECK(d_polys && x && d_out, -1, "poly_eval: null pointer");
     if (batch == 0) return 0;
     std::vector<Fr> xv(batch);
     memcpy(xv.data(), x, sizeof(Fr) * batch);
-    StreamScope ss(c, stream);
-    int rc = poly_eval(reinterpret_cast<const Fr*>(d_polys), stride, n, xv.data(), reinterpret_cast<Fr*>(d_out), (int)batch, c->poly_ws, ss.st);
-    if (!rc && n) g_launches += 2;
-    return rc;
+    return poly_eval(reinterpret_cast<const Fr*>(d_polys), stride, n, xv.data(), reinterpret_cast<Fr*>(d_out), (int)batch, c->poly_ws, st);
+}
+int b200_poly_eval_batch_dev(const void* d_polys, size_t stride, size_t n, const b200_fr* x, size_t batch, void* d_out, void* stream) {
+    B200_ENTER(c, d_polys); StreamScope ss(c, stream);
+    return eval_batch_on(c, ss.st, d_polys, stride, n, x, batch, d_out);
 }
 int b200_poly_eval_batch(const b200_fr* const* polys, size_t n, const b200_fr* x, size_t batch, b200_fr* out) {
     B200_ENTER(c, nullptr);
@@ -1076,75 +1070,67 @@ int b200_poly_eval_batch(const b200_fr* const* polys, size_t n, const b200_fr* x
         B200_CHECK(n == 0 || polys[p], -1, "poly_eval: polys[%zu] is null", p);
         up[p] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[p]), sizeof(Fr) * n};
     }
-    if (n) { if (int rc = h2d_segments(c, c->stage_a.p, up.data(), batch, c->stream)) return rc; }
-    if (int rc = b200_poly_eval_batch_dev(c->stage_a.p, n, n, x, batch, c->small.p, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(out, c->small.p, sizeof(Fr) * batch, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (n) { if (int rc = h2d_segments(c, c->stage_a.p, up.data(), batch, ss.st)) return rc; }
+    if (int rc = eval_batch_on(c, ss.st, c->stage_a.p, n, n, x, batch, c->small.p)) return rc;
+    return d2h_one(c, out, c->small.p, sizeof(Fr) * batch, ss.st);
 }
 int b200_poly_eval(const b200_fr* coeffs, size_t n, const b200_fr* x, b200_fr* out) {
     const b200_fr* p[1] = {coeffs};
     return b200_poly_eval_batch(p, n, x, 1, out);
 }
-int b200_batch_invert_dev(void* d_a, size_t n, void* stream) {
-    B200_ENTER(c, d_a);
+static int batch_invert_on(Ctx* c, cudaStream_t st, void* d_a, size_t n) {
     B200_CHECK(d_a, -1, "batch_invert: null pointer");
-    StreamScope ss(c, stream);
-    int rc = poly_batch_invert(reinterpret_cast<Fr*>(d_a), n, c->poly_ws, ss.st);
-    if (!rc && n) g_launches += 1;
-    return rc;
+    return poly_batch_invert(reinterpret_cast<Fr*>(d_a), n, c->poly_ws, st);
+}
+int b200_batch_invert_dev(void* d_a, size_t n, void* stream) {
+    B200_ENTER(c, d_a); StreamScope ss(c, stream);
+    return batch_invert_on(c, ss.st, d_a, n);
 }
 int b200_batch_invert(b200_fr* a, size_t n) {
     B200_ENTER(c, nullptr);
     B200_CHECK(a, -1, "batch_invert: null pointer");
     if (n == 0) return 0;
     if (c->stage_a.ensure(sizeof(Fr) * n)) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, a, sizeof(Fr) * n, cudaMemcpyHostToDevice, c->stream));
-    if (int rc = b200_batch_invert_dev(c->stage_a.p, n, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(a, c->stage_a.p, sizeof(Fr) * n, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_one(c, c->stage_a.p, a, sizeof(Fr) * n, ss.st)) return rc;
+    if (int rc = batch_invert_on(c, ss.st, c->stage_a.p, n)) return rc;
+    return d2h_one(c, a, c->stage_a.p, sizeof(Fr) * n, ss.st);
 }
-int b200_prefix_scan_dev(int product, const void* d_a, size_t n, const b200_fr* init, void* d_out, void* stream) {
-    B200_ENTER(c, d_a);
-    B200_CHECK(d_a && init && d_out, -1, "prefix_scan: null pointer");
-    const Fr iv = as_fr(init);
-    StreamScope ss(c, stream);
-    int rc = poly_prefix_scan(product != 0, reinterpret_cast<const Fr*>(d_a), n, n, &iv, reinterpret_cast<Fr*>(d_out), n, 1, c->poly_ws, ss.st);
-    if (!rc && n) g_launches += 3;
-    return rc;
-}
-int b200_prefix_scan_batch_dev(int product, const void* d_a, size_t a_stride, size_t n, size_t batch, const b200_fr* inits, void* d_out, size_t out_stride, void* stream) {
-    B200_ENTER(c, d_a);
+static int prefix_scan_on(Ctx* c, cudaStream_t st, int product, const void* d_a, size_t a_stride, size_t n, size_t batch, const b200_fr* inits, void* d_out, size_t out_stride) {
     B200_CHECK(d_a && inits && d_out, -1, "prefix_scan: null pointer");
     B200_CHECK(batch <= 1 || (a_stride >= n && out_stride >= n), -1, "prefix_scan: column stride smaller than the column");
     if (batch == 0) return 0;
     std::vector<Fr> iv(batch);
     memcpy(iv.data(), inits, sizeof(Fr) * batch);
-    StreamScope ss(c, stream);
-    int rc = poly_prefix_scan(product != 0, reinterpret_cast<const Fr*>(d_a), a_stride, n, iv.data(), reinterpret_cast<Fr*>(d_out), out_stride, (int)batch, c->poly_ws, ss.st);
-    if (!rc && n) g_launches += 3;
-    return rc;
+    return poly_prefix_scan(product != 0, reinterpret_cast<const Fr*>(d_a), a_stride, n, iv.data(), reinterpret_cast<Fr*>(d_out), out_stride, (int)batch, c->poly_ws, st);
+}
+int b200_prefix_scan_dev(int product, const void* d_a, size_t n, const b200_fr* init, void* d_out, void* stream) {
+    B200_ENTER(c, d_a); StreamScope ss(c, stream);
+    return prefix_scan_on(c, ss.st, product, d_a, n, n, 1, init, d_out, n);
+}
+int b200_prefix_scan_batch_dev(int product, const void* d_a, size_t a_stride, size_t n, size_t batch, const b200_fr* inits, void* d_out, size_t out_stride, void* stream) {
+    B200_ENTER(c, d_a); StreamScope ss(c, stream);
+    return prefix_scan_on(c, ss.st, product, d_a, a_stride, n, batch, inits, d_out, out_stride);
 }
 int b200_prefix_scan(int product, const b200_fr* a, size_t n, const b200_fr* init, b200_fr* out) {
     B200_ENTER(c, nullptr);
     B200_CHECK(a && init && out, -1, "prefix_scan: null pointer");
     if (n == 0) return 0;
     if (c->stage_a.ensure(sizeof(Fr) * n) || c->stage_b.ensure(sizeof(Fr) * n)) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, a, sizeof(Fr) * n, cudaMemcpyHostToDevice, c->stream));
-    if (int rc = b200_prefix_scan_dev(product, c->stage_a.p, n, init, c->stage_b.p, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(out, c->stage_b.p, sizeof(Fr) * n, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_one(c, c->stage_a.p, a, sizeof(Fr) * n, ss.st)) return rc;
+    if (int rc = prefix_scan_on(c, ss.st, product, c->stage_a.p, n, n, 1, init, c->stage_b.p, n)) return rc;
+    return d2h_one(c, out, c->stage_b.p, sizeof(Fr) * n, ss.st);
 }
-int b200_kate_division_dev(const void* d_a, size_t n, const b200_fr* b, void* d_q, void* stream) {
-    B200_ENTER(c, d_a);
+static int kate_division_on(Ctx* c, cudaStream_t st, const void* d_a, size_t n, const b200_fr* b, void* d_q) {
     B200_CHECK(d_a && b && d_q, -1, "kate_division: null pointer");
     const Fr bv = as_fr(b);
-    StreamScope ss(c, stream);
-    int rc = poly_kate_division(reinterpret_cast<const Fr*>(d_a), n, &bv, reinterpret_cast<Fr*>(d_q), c->poly_ws, ss.st);
-    if (!rc && n > 1) g_launches += 3;
-    return rc;
+    return poly_kate_division(reinterpret_cast<const Fr*>(d_a), n, &bv, reinterpret_cast<Fr*>(d_q), c->poly_ws, st);
+}
+int b200_kate_division_dev(const void* d_a, size_t n, const b200_fr* b, void* d_q, void* stream) {
+    B200_ENTER(c, d_a); StreamScope ss(c, stream);
+    return kate_division_on(c, ss.st, d_a, n, b, d_q);
 }
 int b200_kate_division(const b200_fr* a, size_t n, const b200_fr* b, b200_fr* q) {
     B200_ENTER(c, nullptr);
@@ -1152,61 +1138,64 @@ int b200_kate_division(const b200_fr* a, size_t n, const b200_fr* b, b200_fr* q)
     B200_CHECK(n >= 1, -1, "kate_division: empty polynomial");
     if (n == 1) return 0;
     if (c->stage_a.ensure(sizeof(Fr) * n) || c->stage_b.ensure(sizeof(Fr) * n)) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, a, sizeof(Fr) * n, cudaMemcpyHostToDevice, c->stream));
-    if (int rc = b200_kate_division_dev(c->stage_a.p, n, b, c->stage_b.p, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(q, c->stage_b.p, sizeof(Fr) * (n - 1), cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_one(c, c->stage_a.p, a, sizeof(Fr) * n, ss.st)) return rc;
+    if (int rc = kate_division_on(c, ss.st, c->stage_a.p, n, b, c->stage_b.p)) return rc;
+    return d2h_one(c, q, c->stage_b.p, sizeof(Fr) * (n - 1), ss.st);
 }
 
 // ---- mv-lookup multiplicities --------------------------------------------------------------------------------------------------
-int b200_lookup_multiplicities_dev(const void* d_table, size_t n_table, const void* const* d_inputs, size_t n_inputs, size_t n_rows, void* d_m, uint64_t* missing, void* stream) {
-    B200_ENTER(c, d_table);
+static int lookup_multiplicities_on(Ctx* c, cudaStream_t st, const void* d_table, size_t n_table, const void* const* d_inputs, size_t n_inputs, size_t n_rows, void* d_m,
+                                    uint64_t* missing) {
     B200_CHECK(d_table && d_m && d_inputs && n_inputs >= 1, -1, "lookup_multiplicities: null pointer");
-    StreamScope ss(c, stream);
-    const void* d_ptrs = c->ring.push(d_inputs, sizeof(void*) * n_inputs, ss.st);
+    const void* d_ptrs = c->ring.push(d_inputs, sizeof(void*) * n_inputs, st);
     if (!d_ptrs) {
         if (c->small.ensure(sizeof(void*) * n_inputs)) return -2;
-        B200_CUDA(cudaMemcpyAsync(c->small.p, d_inputs, sizeof(void*) * n_inputs, cudaMemcpyHostToDevice, ss.st));
-        B200_CUDA(cudaStreamSynchronize(ss.st));
+        B200_CUDA(cudaMemcpyAsync(c->small.p, d_inputs, sizeof(void*) * n_inputs, cudaMemcpyHostToDevice, st));
+        B200_CUDA(cudaStreamSynchronize(st));
         d_ptrs = c->small.p;
     }
     unsigned long long* d_missing = nullptr;
     if (int rc = lookup_multiplicities_run(reinterpret_cast<const Fr*>(d_table), n_table, reinterpret_cast<const Fr* const*>(d_ptrs), n_inputs, n_rows,
-                                           reinterpret_cast<Fr*>(d_m), c->msm_ws.misc, &d_missing, ss.st)) return rc;
-    g_launches += 3;
+                                           reinterpret_cast<Fr*>(d_m), c->msm_ws.misc, &d_missing, st)) return rc;
     if (missing) {
         unsigned long long h = 0;
-        B200_CUDA(cudaMemcpyAsync(&h, d_missing, sizeof h, cudaMemcpyDeviceToHost, ss.st));
-        B200_CUDA(cudaStreamSynchronize(ss.st));
+        B200_CUDA(cudaMemcpyAsync(&h, d_missing, sizeof h, cudaMemcpyDeviceToHost, st));
+        B200_CUDA(cudaStreamSynchronize(st));
         *missing = h;
     }
     return 0;
+}
+int b200_lookup_multiplicities_dev(const void* d_table, size_t n_table, const void* const* d_inputs, size_t n_inputs, size_t n_rows, void* d_m, uint64_t* missing, void* stream) {
+    B200_ENTER(c, d_table); StreamScope ss(c, stream);
+    return lookup_multiplicities_on(c, ss.st, d_table, n_table, d_inputs, n_inputs, n_rows, d_m, missing);
 }
 int b200_lookup_multiplicities(const b200_fr* table, size_t n_table, const b200_fr* const* inputs, size_t n_inputs, size_t n_rows, b200_fr* m, uint64_t* missing) {
     B200_ENTER(c, nullptr);
     B200_CHECK(table && inputs && m && n_inputs >= 1, -1, "lookup_multiplicities: null pointer");
     if (c->stage_a.ensure(sizeof(Fr) * (n_table + n_inputs * (n_rows ? n_rows : 1))) || c->stage_b.ensure(sizeof(Fr) * n_table)) return -2;
-    B200_CUDA(cudaMemcpyAsync(c->stage_a.p, table, sizeof(Fr) * n_table, cudaMemcpyHostToDevice, c->stream));
+    // the table and then every input column, back to back in stage_a
     std::vector<const void*> ptrs(n_inputs);
+    std::vector<HostSeg> up(1 + (n_rows ? n_inputs : 0));
+    up[0] = HostSeg{(uint8_t*)const_cast<b200_fr*>(table), sizeof(Fr) * n_table};
     for (size_t j = 0; j < n_inputs; ++j) {
         B200_CHECK(inputs[j] || n_rows == 0, -1, "lookup_multiplicities: inputs[%zu] is null", j);
         ptrs[j] = c->stage_a.as<Fr>() + n_table + j * n_rows;
-        if (n_rows) B200_CUDA(cudaMemcpyAsync(const_cast<void*>(ptrs[j]), inputs[j], sizeof(Fr) * n_rows, cudaMemcpyHostToDevice, c->stream));
+        if (n_rows) up[1 + j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(inputs[j]), sizeof(Fr) * n_rows};
     }
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), ss.st)) return rc;
     uint64_t miss = 0;
-    if (int rc = b200_lookup_multiplicities_dev(c->stage_a.p, n_table, ptrs.data(), n_inputs, n_rows, c->stage_b.p, &miss, nullptr)) return rc;
-    B200_CUDA(cudaMemcpyAsync(m, c->stage_b.p, sizeof(Fr) * n_table, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
+    if (int rc = lookup_multiplicities_on(c, ss.st, c->stage_a.p, n_table, ptrs.data(), n_inputs, n_rows, c->stage_b.p, &miss)) return rc;
+    if (int rc = d2h_one(c, m, c->stage_b.p, sizeof(Fr) * n_table, ss.st)) return rc;
     if (missing) *missing = miss;
     return 0;
 }
 
 // ---- quotient numerator (evaluate_h) ------------------------------------------------------------------------------
 static_assert(sizeof(b200_instr) == sizeof(QInstr) && sizeof(b200_col_ref) == sizeof(QLoad), "ABI structs must match the kernel's");
-int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
-                           const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out, void* stream) {
-    B200_ENTER(c, d_out);
+static int quotient_eval_on(Ctx* c, cudaStream_t st, const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
+                            const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out) {
     B200_CHECK(d_out && (n_columns == 0 || d_columns) && (n_loads == 0 || loads) && (n_constants == 0 || constants) && (n_instr == 0 || program), -1, "quotient_eval: null pointer");
     B200_CHECK(ext_k >= k && ext_k <= 28, -1, "quotient_eval: need k <= ext_k <= 28");
     const uint64_t N = 1ull << ext_k, scale = 1ull << (ext_k - k);
@@ -1216,11 +1205,13 @@ int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint3
         const int64_t off = (int64_t)loads[i].rotation * (int64_t)scale;           // Rotation(r) on the extended domain = r * 2^(ext_k - k)
         ql[i].offset = (uint32_t)(((off % (int64_t)N) + (int64_t)N) % (int64_t)N);
     }
-    StreamScope ss(c, stream);
-    int rc = quotient_eval_run(reinterpret_cast<const Fr* const*>(d_columns), n_columns, ext_k, ql.data(), n_loads, reinterpret_cast<const Fr*>(constants), n_constants,
-                               reinterpret_cast<const QInstr*>(program), n_instr, reinterpret_cast<Fr*>(d_out), c->quot_ws, ss.st);
-    if (!rc) g_launches += 1;
-    return rc;
+    return quotient_eval_run(reinterpret_cast<const Fr* const*>(d_columns), n_columns, ext_k, ql.data(), n_loads, reinterpret_cast<const Fr*>(constants), n_constants,
+                             reinterpret_cast<const QInstr*>(program), n_instr, reinterpret_cast<Fr*>(d_out), c->quot_ws, st);
+}
+int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
+                           const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out, void* stream) {
+    B200_ENTER(c, d_out); StreamScope ss(c, stream);
+    return quotient_eval_on(c, ss.st, d_columns, n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, d_out);
 }
 int b200_quotient_eval(const b200_fr* const* columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
                        const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, b200_fr* out) {
@@ -1236,9 +1227,10 @@ int b200_quotient_eval(const b200_fr* const* columns, size_t n_columns, uint32_t
         ptrs[i] = c->stage_a.as<Fr>() + i * N;
         up[i] = HostSeg{(uint8_t*)const_cast<b200_fr*>(columns[i]), sizeof(Fr) * N};
     }
-    if (int rc = h2d_segments(c, c->stage_a.p, up.data(), n_columns, c->stream)) return rc;
-    if (int rc = b200_quotient_eval_dev(ptrs.data(), n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, c->stage_b.p, nullptr)) return rc;
-    return d2h_one(c, out, c->stage_b.p, sizeof(Fr) * N, c->stream);
+    StreamScope ss(c, nullptr);
+    if (int rc = h2d_segments(c, c->stage_a.p, up.data(), n_columns, ss.st)) return rc;
+    if (int rc = quotient_eval_on(c, ss.st, ptrs.data(), n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, c->stage_b.p)) return rc;
+    return d2h_one(c, out, c->stage_b.p, sizeof(Fr) * N, ss.st);
 }
 
 // evaluate_h at its natural boundary: the CPU evaluator receives coefficient-form polynomials and builds their cosets itself
@@ -1280,7 +1272,7 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
         while (p0 < group.size()) {
             size_t p1 = p0 + 1;
             while (p1 < group.size() && group[p1] == group[p1 - 1] + 1) ++p1;
-            if (int rc = ntt_call(c, c->stage_a.as<Fr>() + p0 * len, len, len, c->stage_b.as<Fr>(), ext + group[p0] * N, N, ext_k, as_fr(ext_omega), pre, none, (int)(p1 - p0), ss.st)) return rc;
+            if (int rc = ntt_call(c, ss.st, c->stage_a.as<Fr>() + p0 * len, len, len, c->stage_b.as<Fr>(), ext + group[p0] * N, N, ext_k, as_fr(ext_omega), pre, none, (int)(p1 - p0))) return rc;
             p0 = p1;
         }
         B200_CUDA(cudaStreamSynchronize(ss.st));          // the coefficient staging buffer is reused by the next group
@@ -1298,13 +1290,13 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
     std::vector<const void*> ptrs(n_columns);
     for (size_t i = 0; i < n_columns; ++i) ptrs[i] = ext + i * N;
     Fr* h = c->stage_b.as<Fr>();
-    if (int rc = b200_quotient_eval_dev(ptrs.data(), n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, h, ss.st)) return rc;
+    if (int rc = quotient_eval_on(c, ss.st, ptrs.data(), n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, h)) return rc;
     if (t_evaluations) {
-        if (int rc = b200_poly_scale_cycle_dev(h, N, t_evaluations, t_period, ss.st)) return rc;
+        if (int rc = scale_cycle_on(c, ss.st, h, N, t_evaluations, t_period)) return rc;
         NttScale post;
         const Fr z = as_fr(zeta), z2 = z * z, d = as_fr(ext_ifft_divisor);
         post.mode = 3; post.c[0] = d; post.c[1] = d * z2; post.c[2] = d * z;
-        if (int rc = ntt_call(c, h, N, N, ext, h, N, ext_k, as_fr(ext_omega_inv), none, post, 1, ss.st)) return rc;      // `ext` is free again: scratch
+        if (int rc = ntt_call(c, ss.st, h, N, N, ext, h, N, ext_k, as_fr(ext_omega_inv), none, post, 1)) return rc;      // `ext` is free again: scratch
     }
     return d2h_one(c, out, h, sizeof(Fr) * N, ss.st);
 }

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <atomic>
 #include <string>
 
 namespace b200 {
@@ -11,6 +12,12 @@ namespace b200 {
 // Thread-local last-error string behind b200_last_error() (include/ezkl_b200.h).
 void set_error(const char* fmt, ...);
 const char* get_error();
+
+// Kernels launched by libezkl_b200.so since load (b200_launch_count): every launch site of the operation kernels calls
+// count_launch() right after issuing its launch, so a launch that then fails is counted too.  The test-only debug library
+// (debug.cu, libezkl_b200_dbg.so) has its own copy of this counter, which nothing reads.
+inline std::atomic<uint64_t> g_launches{0};
+inline void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 #define B200_CUDA(call)                                                                                  \
     do {                                                                                                 \

@@ -64,13 +64,12 @@ int g1_fft_run(const G1Affine* d_in, uint32_t log_n, const Fr& omega, const Fr* 
     if (scratch.ensure(sizeof(G1Xyzz) * n + sizeof(Fr) * half)) return -2;
     G1Xyzz* work = scratch.as<G1Xyzz>();
     Fr* tw = reinterpret_cast<Fr*>(work + n);
-    k_powers_fr<<<div_up(half, 128), 128, 0, st>>>(omega, (uint32_t)half, tw);
-    k_ecfft_load<<<div_up(n, 64), 64, 0, st>>>(d_in, log_n, scale ? *scale : fp_one<FrTag>(), scale ? 1 : 0, work);
-    for (uint32_t log_h = 0; log_h < log_n; ++log_h) k_ecfft_stage<<<div_up(n / 2, 64), 64, 0, st>>>(work, log_n, log_h, tw);
-    k_ecfft_store<<<div_up(n, 128), 128, 0, st>>>(work, n, d_out);
+    k_powers_fr<<<div_up(half, 128), 128, 0, st>>>(omega, (uint32_t)half, tw); count_launch();
+    k_ecfft_load<<<div_up(n, 64), 64, 0, st>>>(d_in, log_n, scale ? *scale : fp_one<FrTag>(), scale ? 1 : 0, work); count_launch();
+    for (uint32_t log_h = 0; log_h < log_n; ++log_h) { k_ecfft_stage<<<div_up(n / 2, 64), 64, 0, st>>>(work, log_n, log_h, tw); count_launch(); }
+    k_ecfft_store<<<div_up(n, 128), 128, 0, st>>>(work, n, d_out); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
-int g1_fft_launches(uint32_t log_n) { return 3 + (int)log_n; }
 
 }  // namespace b200

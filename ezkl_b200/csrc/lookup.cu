@@ -76,13 +76,13 @@ int lookup_multiplicities_run(const Fr* d_table, size_t n_table, const Fr* const
     unsigned long long* missing = reinterpret_cast<unsigned long long*>(scratch.as<uint8_t>() + ((sizeof(uint32_t) * ((size_t)cap + n_table) + 7) & ~(size_t)7));
     B200_CUDA(cudaMemsetAsync(slots, 0xff, sizeof(uint32_t) * cap, st));
     B200_CUDA(cudaMemsetAsync(counts, 0, sizeof(uint32_t) * n_table + 16, st));
-    k_lk_build<<<div_up(n_table, 256), 256, 0, st>>>(d_table, (uint32_t)n_table, slots, cap - 1);
+    k_lk_build<<<div_up(n_table, 256), 256, 0, st>>>(d_table, (uint32_t)n_table, slots, cap - 1); count_launch();
     if (n_rows) {
         const unsigned gmax = (unsigned)sm_count() * 8u;
         const unsigned gx = div_up(n_rows, 256) > gmax ? gmax : div_up(n_rows, 256);
-        k_lk_count<<<dim3(gx, (unsigned)n_inputs), 256, 0, st>>>(d_table, slots, cap - 1, d_inputs, (uint32_t)n_rows, counts, missing);
+        k_lk_count<<<dim3(gx, (unsigned)n_inputs), 256, 0, st>>>(d_table, slots, cap - 1, d_inputs, (uint32_t)n_rows, counts, missing); count_launch();
     }
-    k_lk_finish<<<div_up(n_table, 256), 256, 0, st>>>(counts, (uint32_t)n_table, d_m);
+    k_lk_finish<<<div_up(n_table, 256), 256, 0, st>>>(counts, (uint32_t)n_table, d_m); count_launch();
     B200_CUDA(cudaGetLastError());
     *d_missing_out = missing;
     return 0;

@@ -33,7 +33,6 @@ int msm_default_window(size_t n) {
     if (c > 22) c = 22;
     return c;
 }
-int msm_launches_per_run() { return 11; }
 
 // ---------------------------------------------------------------------------------------------------------
 // table precomputation
@@ -57,7 +56,7 @@ int msm_table_build(MsmTable* t, const G1Affine* d_bases, size_t n, int c, cudaS
     B200_CUDA(cudaMalloc(&t->d_table, sizeof(G1Affine) * n * W));
     B200_CUDA(cudaMemcpyAsync(t->d_table, d_bases, sizeof(G1Affine) * n, cudaMemcpyDeviceToDevice, st));
     for (int w = 1; w < W; ++w) {
-        k_table_next_level<<<div_up(n, 128), 128, 0, st>>>(t->d_table + (size_t)(w - 1) * n, t->d_table + (size_t)w * n, n, c);
+        k_table_next_level<<<div_up(n, 128), 128, 0, st>>>(t->d_table + (size_t)(w - 1) * n, t->d_table + (size_t)w * n, n, c); count_launch();
     }
     B200_CUDA(cudaGetLastError());
     return 0;
@@ -421,7 +420,7 @@ __global__ void __launch_bounds__(128) k_g1_generate(uint64_t seed, size_t n, G1
 }
 int g1_generate_run(uint64_t seed, size_t n, G1Affine* d_out, cudaStream_t st) {
     if (n == 0) return 0;
-    k_g1_generate<<<div_up(n, 128), 128, 0, st>>>(seed, n, d_out);
+    k_g1_generate<<<div_up(n, 128), 128, 0, st>>>(seed, n, d_out); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -441,7 +440,7 @@ __global__ void __launch_bounds__(128) k_g1_fixed_base_mul(const Fr* __restrict_
 }
 int g1_fixed_base_mul_run(const Fr* d_scalars, size_t n, const G1Affine& base, G1Affine* d_out, cudaStream_t st) {
     if (n == 0) return 0;
-    k_g1_fixed_base_mul<<<div_up(n, 128), 128, 0, st>>>(d_scalars, n, base, d_out);
+    k_g1_fixed_base_mul<<<div_up(n, 128), 128, 0, st>>>(d_scalars, n, base, d_out); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -449,7 +448,7 @@ int g1_fixed_base_mul_run(const Fr* d_scalars, size_t n, const G1Affine& base, G
 int g1_sum_run(const G1Xyzz* d_points, size_t groups, size_t count, G1Xyzz* d_out, cudaStream_t st) {
     if (groups == 0) return 0;
     B200_CHECK(groups <= 0x7fffffffu && count <= 0xffffffffu, -1, "g1_sum: sizes out of range");
-    k_final_coop<<<(unsigned)groups, TREE_THREADS, 0, st>>>(d_points, (uint32_t)count, d_out);
+    k_final_coop<<<(unsigned)groups, TREE_THREADS, 0, st>>>(d_points, (uint32_t)count, d_out); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -539,28 +538,28 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     const unsigned sms = (unsigned)sm_count();
     const unsigned dig_blocks = min(div_up(n, 256), sms * 8u);
     dim3 gd(dig_blocks, batch);
-    k_digits<false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr);
-    k_scan_buckets<<<batch, 1024, 0, st>>>(hist, offs, chunk_offs, nb, cap, skew);
-    k_digits<true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew);
-    k_fill_chunks<<<dim3(div_up(nb, 256), batch), 256, (cap + 1) * 4, st>>>(offs, chunk_offs, nb, cap, chunk_start, chunk_len, chunk_stride, len_hist, heavy, heavy_stride);
-    k_len_offsets<<<batch, 32, 0, st>>>(len_hist, len_offs, cap);
+    k_digits<false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr); count_launch();
+    k_scan_buckets<<<batch, 1024, 0, st>>>(hist, offs, chunk_offs, nb, cap, skew); count_launch();
+    k_digits<true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew); count_launch();
+    k_fill_chunks<<<dim3(div_up(nb, 256), batch), 256, (cap + 1) * 4, st>>>(offs, chunk_offs, nb, cap, chunk_start, chunk_len, chunk_stride, len_hist, heavy, heavy_stride); count_launch();
+    k_len_offsets<<<batch, 32, 0, st>>>(len_hist, len_offs, cap); count_launch();
     const unsigned ch_blocks = min(div_up(chunk_stride, 256), sms * 8u);
-    k_order_chunks<<<dim3(ch_blocks, batch), 256, 0, st>>>(chunk_len, chunk_stride, chunk_offs, nb, len_offs, len_cursor, cap, order);
+    k_order_chunks<<<dim3(ch_blocks, batch), 256, 0, st>>>(chunk_len, chunk_stride, chunk_offs, nb, len_offs, len_cursor, cap, order); count_launch();
     if (prof_enabled()) prof_mark(PROF_MSM_RECODE, st, false);
     const unsigned acc_blocks = min(div_up(chunk_stride, 128), sms * 16u);
     {
         ProfScope ps(PROF_MSM_ACCUMULATE, st);
-        k_accumulate<<<dim3(acc_blocks, batch), 128, 0, st>>>(t.d_table, ents, ent_stride, chunk_start, chunk_len, order, chunk_stride, chunk_offs, nb, chunk_sums);
+        k_accumulate<<<dim3(acc_blocks, batch), 128, 0, st>>>(t.d_table, ents, ent_stride, chunk_start, chunk_len, order, chunk_stride, chunk_offs, nb, chunk_sums); count_launch();
     }
     ProfScope ps_tail(PROF_MSM_TAIL, st);
-    k_combine<<<dim3(div_up(nb, 128), batch), 128, 0, st>>>(chunk_offs, nb, chunk_sums, chunk_stride, bucket_sums);
-    k_combine_heavy<<<dim3(32, batch), TREE_THREADS, 0, st>>>(heavy, heavy_stride, chunk_offs, nb, chunk_sums, chunk_stride, bucket_sums);
+    k_combine<<<dim3(div_up(nb, 128), batch), 128, 0, st>>>(chunk_offs, nb, chunk_sums, chunk_stride, bucket_sums); count_launch();
+    k_combine_heavy<<<dim3(32, batch), TREE_THREADS, 0, st>>>(heavy, heavy_stride, chunk_offs, nb, chunk_sums, chunk_stride, bucket_sums); count_launch();
     if (coop) {
-        k_reduce_coop<<<dim3(nparts, batch), TREE_THREADS, 0, st>>>(bucket_sums, nb, partials, nparts, reduce_m);
-        k_final_coop<<<batch, TREE_THREADS, 0, st>>>(partials, nparts, d_out);
+        k_reduce_coop<<<dim3(nparts, batch), TREE_THREADS, 0, st>>>(bucket_sums, nb, partials, nparts, reduce_m); count_launch();
+        k_final_coop<<<batch, TREE_THREADS, 0, st>>>(partials, nparts, d_out); count_launch();
     } else {
-        k_reduce<1><<<dim3(nparts, batch), reduce_threads, 0, st>>>(bucket_sums, nb, partials, nparts, reduce_m);
-        k_final<<<batch, final_threads, 0, st>>>(partials, nparts, d_out);
+        k_reduce<1><<<dim3(nparts, batch), reduce_threads, 0, st>>>(bucket_sums, nb, partials, nparts, reduce_m); count_launch();
+        k_final<<<batch, final_threads, 0, st>>>(partials, nparts, d_out); count_launch();
     }
     B200_CUDA(cudaGetLastError());
     return 0;

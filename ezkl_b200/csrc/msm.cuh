@@ -31,14 +31,11 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
 int g1_fixed_base_mul_run(const Fr* d_scalars, size_t n, const G1Affine& base, G1Affine* d_out, cudaStream_t st);
 // out[j] = scale * sum_i omega^(i j) * P_i over G1 (halo2 g_to_lagrange / ParamsKZG::downsize); affine in, affine out
 int g1_fft_run(const G1Affine* d_in, uint32_t log_n, const Fr& omega, const Fr* scale, G1Affine* d_out, DevBuf& scratch, cudaStream_t st);
-int g1_fft_launches(uint32_t log_n);
 int g1_generate_run(uint64_t seed, size_t n, G1Affine* d_out, cudaStream_t st);
 // out[g] = sum_j points[g*count + j]
 int g1_sum_run(const G1Xyzz* d_points, size_t groups, size_t count, G1Xyzz* d_out, cudaStream_t st);
 // bytes of workspace msm_run needs per column (upper bound, for batch splitting)
 size_t msm_workspace_per_column(const MsmTable& t, size_t n);
-// number of kernels msm_run launches for one call (for bench.py's gpu_launches accounting)
-int msm_launches_per_run();
 
 // Signed c-bit window recoding of a canonical (non-Montgomery) scalar, one digit per call, low window first:
 // consumes the low c bits of s (s is shifted right in place) and returns a digit in [-2^(c-1), 2^(c-1)].

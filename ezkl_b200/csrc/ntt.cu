@@ -293,7 +293,6 @@ static void choose_passes(uint32_t log_n, int* npass, int logm[3]) {
     *npass = 3;
     logm[0] = (int)(log_n + 2) / 3; logm[1] = (int)(log_n - logm[0] + 1) / 2; logm[2] = (int)log_n - logm[0] - logm[1];
 }
-int ntt_launches_per_run(uint32_t log_n) { int np, lm[3]; choose_passes(log_n, &np, lm); return np; }
 
 static Fr host_pow(const Fr& b, uint64_t e) { return fp_pow_u64(b, e); }
 
@@ -306,7 +305,7 @@ NttPlan* NttContext::get(uint32_t log_n, const Fr& omega, cudaStream_t st) {
     for (int i = 0; i < p->npass; ++i) {
         const uint32_t M = 1u << p->logm[i], cnt = M > 1 ? M / 2 : 1;
         if (cudaMalloc(&p->d_tw[i], sizeof(Fr) * cnt) != cudaSuccess) { set_error("ntt plan: cudaMalloc failed"); delete p; return nullptr; }
-        k_powers<<<div_up(cnt, 128), 128, 0, st>>>(host_pow(omega, N / M), cnt, p->d_tw[i]);
+        k_powers<<<div_up(cnt, 128), 128, 0, st>>>(host_pow(omega, N / M), cnt, p->d_tw[i]); count_launch();
     }
     p->lo_bits = (log_n + 1) / 2;
     const uint32_t nlo = 1u << p->lo_bits, nhi = (uint32_t)(N >> p->lo_bits);
@@ -316,14 +315,14 @@ NttPlan* NttContext::get(uint32_t log_n, const Fr& omega, cudaStream_t st) {
     for (int i = 0; i < p->npass; ++i) {
         const uint32_t M = 1u << p->logm[i];
         if (cudaMalloc(&p->d_staged[i], sizeof(uint4) * 2 * M) != cudaSuccess) { set_error("ntt plan: cudaMalloc failed"); delete p; return nullptr; }
-        k_stage_twiddles<<<div_up(M, 128), 128, 0, st>>>(host_pow(omega, N / M), (uint32_t)p->logm[i], p->d_staged[i]);
+        k_stage_twiddles<<<div_up(M, 128), 128, 0, st>>>(host_pow(omega, N / M), (uint32_t)p->logm[i], p->d_staged[i]); count_launch();
     }
     if (p->npass > 1 && log_n <= 25) {        // full single-multiply twiddle table (N * 32 B; falls back to the two-level table if it does not fit)
         if (cudaMalloc(&p->d_full, sizeof(Fr) * N) != cudaSuccess) { cudaGetLastError(); p->d_full = nullptr; }
-        else k_powers_run<<<div_up(div_up(N, 32), 128), 128, 0, st>>>(omega, N, p->d_full);
+        else { k_powers_run<<<div_up(div_up(N, 32), 128), 128, 0, st>>>(omega, N, p->d_full); count_launch(); }
     }
-    k_powers<<<div_up(nlo, 128), 128, 0, st>>>(omega, nlo, p->d_lo);
-    k_powers<<<div_up(nhi ? nhi : 1, 128), 128, 0, st>>>(host_pow(omega, 1ull << p->lo_bits), nhi ? nhi : 1, p->d_hi);
+    k_powers<<<div_up(nlo, 128), 128, 0, st>>>(omega, nlo, p->d_lo); count_launch();
+    k_powers<<<div_up(nhi ? nhi : 1, 128), 128, 0, st>>>(host_pow(omega, 1ull << p->lo_bits), nhi ? nhi : 1, p->d_hi); count_launch();
     if (cudaGetLastError() != cudaSuccess) { set_error("ntt plan: table kernel launch failed"); delete p; return nullptr; }
     plans.push_back(p);
     return p;
@@ -363,7 +362,7 @@ static int launch_pass(PassArgs& a, uint64_t lines, int batch, cudaStream_t st) 
     B200_CHECK(threads <= 256 && smem <= 200 * 1024, -1, "ntt: pass of 2^%u does not fit a CTA", a.logm);
     B200_CUDA(cudaFuncSetAttribute(k_ntt_pass2, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     // per device, idempotent
     dim3 grid((unsigned)(lines >> a.log_g), (unsigned)batch);
-    k_ntt_pass2<<<grid, threads, smem, st>>>(a);
+    k_ntt_pass2<<<grid, threads, smem, st>>>(a); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -383,7 +382,7 @@ static int launch_pass_v1(PassArgs& a, uint64_t lines, int batch, cudaStream_t s
     if (cfg.ntt_threads >= 32 && cfg.ntt_threads <= 1024 && (uint32_t)cfg.ntt_threads < threads) threads = (uint32_t)cfg.ntt_threads;
     B200_CUDA(cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     // per device, idempotent
     dim3 grid((unsigned)(lines >> log_g), (unsigned)batch);
-    k_ntt_pass<<<grid, threads, smem, st>>>(a);
+    k_ntt_pass<<<grid, threads, smem, st>>>(a); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -482,7 +481,7 @@ int ntt_run_sharded(NttPlan* const* plans, int ndev, const int* dev_ids, const F
             for (int h = 0; h < ndev; ++h) { a.src_peers[h] = bufs_r[r.in_buf][h]; a.dst_peers[h] = const_cast<Fr*>(bufs_r[r.out_buf][h]); }
             B200_CUDA(cudaSetDevice(dev_ids[g]));
             B200_CUDA(cudaFuncSetAttribute(k_ntt_pass2, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-            k_ntt_pass2<<<dim3((unsigned)(blocks / ndev), 1), threads, smem, st[g]>>>(a);
+            k_ntt_pass2<<<dim3((unsigned)(blocks / ndev), 1), threads, smem, st[g]>>>(a); count_launch();
             B200_CUDA(cudaGetLastError());
             B200_CUDA(cudaEventRecord(ev[g], st[g]));
         }

@@ -38,7 +38,6 @@ struct NttContext {
 // dst may alias src (when n_in == 2^log_n and strides match); tmp must not alias either.
 int ntt_run(NttPlan* plan, const Fr* d_src, size_t src_stride, size_t n_in, Fr* d_tmp, size_t tmp_stride, Fr* d_dst, size_t dst_stride,
             uint32_t log_n, const Fr& omega, const NttScale& pre, const NttScale& post, int batch, cudaStream_t st);
-int ntt_launches_per_run(uint32_t log_n);
 // one transform split across devices in contiguous natural-order slices, exchanges fused into the passes (ntt.cu)
 int ntt_run_sharded(NttPlan* const* plans, int ndev, const int* dev_ids, const Fr* const* src, Fr* const* tmp, Fr* const* dst, uint32_t log_n, const Fr& omega,
                     const NttScale& pre, const NttScale& post, uint64_t n_in, cudaStream_t* st, cudaEvent_t* ev);

@@ -47,7 +47,7 @@ static unsigned ew_grid(size_t n) { const unsigned gmax = (unsigned)sm_count() *
 int poly_binary(int op, const Fr* a, const Fr* b, const Fr* h_s, Fr* out, size_t n, cudaStream_t st) {
     if (n == 0) return 0;
     Fr s = h_s ? *h_s : fp_zero<FrTag>();
-    k_poly_binary<<<ew_grid(n), 256, 0, st>>>(op, a, b, s, out, n);
+    k_poly_binary<<<ew_grid(n), 256, 0, st>>>(op, a, b, s, out, n); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -64,14 +64,14 @@ int poly_lincomb(const Fr* const* h_polys /*device addresses*/, const Fr* h_scal
         B200_CUDA(cudaStreamSynchronize(st));
         d = ws.scratch.as<uint8_t>();
     }
-    k_poly_lincomb<<<ew_grid(n), 256, 0, st>>>(reinterpret_cast<const Fr* const*>(d), reinterpret_cast<const Fr*>(d + o_s), (uint32_t)count, out, n);
+    k_poly_lincomb<<<ew_grid(n), 256, 0, st>>>(reinterpret_cast<const Fr* const*>(d), reinterpret_cast<const Fr*>(d + o_s), (uint32_t)count, out, n); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
 int poly_scale_cycle(const Fr* a, const Fr* d_consts, uint32_t period, Fr* out, size_t n, cudaStream_t st) {
     if (n == 0) return 0;
     B200_CHECK(period > 0, -1, "poly_scale_cycle: period 0");
-    k_poly_scale_cycle<<<ew_grid(n), 256, 0, st>>>(a, d_consts, period, out, n);
+    k_poly_scale_cycle<<<ew_grid(n), 256, 0, st>>>(a, d_consts, period, out, n); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -198,8 +198,8 @@ int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_ou
     WArgs* d_w; uint8_t* extra;
     if (int rc = upload_wargs(h_x, batch, ws, sizeof(Fr) * (size_t)nblk * batch, &d_w, &extra, st)) return rc;
     Fr* blk_val = reinterpret_cast<Fr*>(extra);
-    k_wscan_block_values<<<dim3(nblk, batch), TB, 0, st>>>(coeffs, stride, n, d_w, blk_val, nblk);
-    k_wscan_carries<<<batch, carry_threads(nblk), 0, st>>>(blk_val, nblk, d_w, nullptr, d_out);
+    k_wscan_block_values<<<dim3(nblk, batch), TB, 0, st>>>(coeffs, stride, n, d_w, blk_val, nblk); count_launch();
+    k_wscan_carries<<<batch, carry_threads(nblk), 0, st>>>(blk_val, nblk, d_w, nullptr, d_out); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -213,9 +213,9 @@ int poly_kate_division(const Fr* a, size_t n, const Fr* h_b, Fr* q, PolyWorkspac
     if (int rc = upload_wargs(h_b, 1, ws, sizeof(Fr) * (size_t)nblk * 2, &d_w, &extra, st)) return rc;
     Fr* blk_val = reinterpret_cast<Fr*>(extra);
     Fr* carry = blk_val + nblk;
-    k_wscan_block_values<<<dim3(nblk, 1), TB, 0, st>>>(a + 1, 0, m, d_w, blk_val, nblk);
-    k_wscan_carries<<<1, carry_threads(nblk), 0, st>>>(blk_val, nblk, d_w, carry, nullptr);
-    k_wscan_apply<<<nblk, TB, 0, st>>>(a + 1, m, d_w, carry, q);
+    k_wscan_block_values<<<dim3(nblk, 1), TB, 0, st>>>(a + 1, 0, m, d_w, blk_val, nblk); count_launch();
+    k_wscan_carries<<<1, carry_threads(nblk), 0, st>>>(blk_val, nblk, d_w, carry, nullptr); count_launch();
+    k_wscan_apply<<<nblk, TB, 0, st>>>(a + 1, m, d_w, carry, q); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -284,13 +284,13 @@ int poly_prefix_scan(bool product, const Fr* a, size_t a_stride, size_t n, const
     }
     const dim3 grid(nblk, batch);
     if (product) {
-        k_scan_block_totals<true><<<grid, TB, 0, st>>>(a, a_stride, n, blk_tot, nblk);
-        k_scan_block_prefixes<true><<<batch, 1024, 0, st>>>(blk_tot, nblk, staged, blk_pre);
-        k_scan_apply<true><<<grid, TB, 0, st>>>(a, a_stride, n, blk_pre, nblk, out, out_stride);
+        k_scan_block_totals<true><<<grid, TB, 0, st>>>(a, a_stride, n, blk_tot, nblk); count_launch();
+        k_scan_block_prefixes<true><<<batch, 1024, 0, st>>>(blk_tot, nblk, staged, blk_pre); count_launch();
+        k_scan_apply<true><<<grid, TB, 0, st>>>(a, a_stride, n, blk_pre, nblk, out, out_stride); count_launch();
     } else {
-        k_scan_block_totals<false><<<grid, TB, 0, st>>>(a, a_stride, n, blk_tot, nblk);
-        k_scan_block_prefixes<false><<<batch, 1024, 0, st>>>(blk_tot, nblk, staged, blk_pre);
-        k_scan_apply<false><<<grid, TB, 0, st>>>(a, a_stride, n, blk_pre, nblk, out, out_stride);
+        k_scan_block_totals<false><<<grid, TB, 0, st>>>(a, a_stride, n, blk_tot, nblk); count_launch();
+        k_scan_block_prefixes<false><<<batch, 1024, 0, st>>>(blk_tot, nblk, staged, blk_pre); count_launch();
+        k_scan_apply<false><<<grid, TB, 0, st>>>(a, a_stride, n, blk_pre, nblk, out, out_stride); count_launch();
     }
     B200_CUDA(cudaGetLastError());
     return 0;
@@ -321,7 +321,7 @@ int poly_batch_invert(Fr* a, size_t n, PolyWorkspace& ws, cudaStream_t st) {
     if (n == 0) return 0;
     if (ws.scratch.ensure(sizeof(Fr) * n)) return -2;
     const size_t nthreads = (n + INV_CHUNK - 1) / INV_CHUNK;
-    k_batch_invert<<<div_up(nthreads, 128), 128, 0, st>>>(a, ws.scratch.as<Fr>(), n);
+    k_batch_invert<<<div_up(nthreads, 128), 128, 0, st>>>(a, ws.scratch.as<Fr>(), n); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }

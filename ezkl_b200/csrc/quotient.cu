@@ -114,6 +114,7 @@ int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k
     else if (max_slot < 128) B200_QLAUNCH(128);
     else B200_QLAUNCH(256);
 #undef B200_QLAUNCH
+    count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }

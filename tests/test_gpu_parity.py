@@ -558,3 +558,122 @@ def test_batch_splitting_paths():
     env = dict(os.environ, B200_WS_BUDGET_MB="1")
     r = subprocess.run([sys.executable, os.path.join(H.ROOT, "tests", "split_paths_check.py")], capture_output=True, text=True, timeout=600, env=env)
     assert r.returncode == 0 and "split paths OK" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+
+
+def test_host_entry_points_on_the_bounce_path():
+    """Host-buffer entry points with columns above the 24 MiB direct-copy limit, which staging moves through the pinned bounce
+    slots.  n = 2^20 + 3 Fr is 32 MiB + 96 B, so every column ends in a partial 16 MiB slot.  Results against the oracle."""
+    from ezkl_b200 import device as dev
+    from ezkl_b200 import evaluation as ev
+    from ezkl_b200 import fields as F
+    n = (1 << 20) + 3
+    a, b = orc.gen_scalars(n, seed=90), orc.gen_scalars(n, seed=91)
+    s = orc.gen_scalars(1, seed=92)[0]
+    for op in ("add", "sub", "mul"):
+        assert np.array_equal(h2.poly_op(op, a, b), orc.poly_op(op, a, b, threads=THREADS)), op
+    assert np.array_equal(h2.poly_op("scale", a, s=s), orc.poly_op("scale", a, s=s, threads=THREADS))
+    assert np.array_equal(h2.poly_op("axpy", a, b, s), orc.poly_op("axpy", a, b, s, threads=THREADS))
+    assert np.array_equal(h2.eval_polynomial(a, s), orc.eval_polynomial(a, s))
+    assert np.array_equal(h2.kate_division(a, s), orc.kate_division(a, s))
+    z = a.copy()
+    z[::5] = 0
+    assert np.array_equal(h2.batch_invert(z), orc.batch_invert(z))
+    one = orc.fr_one()
+    assert np.array_equal(h2.prefix_scan(a, one, True), orc.prefix_scan(a, one, True))
+    assert np.array_equal(h2.prefix_scan(a, s, False), orc.prefix_scan(a, s, False))
+    # poly_scale_cycle on the ragged length: a * (the period-4 constants repeated)
+    cs = orc.gen_scalars(4, seed=93)
+    got = a.copy()
+    nat.check(nat.lib().b200_poly_scale_cycle(nat.ptr(got), C.c_size_t(n), nat.ptr(cs), C.c_uint32(4)))
+    assert np.array_equal(got, orc.poly_op("mul", a, np.ascontiguousarray(np.tile(cs, ((n + 3) // 4, 1))[:n]), threads=THREADS))
+    dom = h2.EvaluationDomain(5, 18)                      # extended domain 2^20: one 32 MiB column
+    ext = orc.gen_scalars(dom.extended_len(), seed=94)
+    assert np.array_equal(dom.divide_by_vanishing_poly(ext), orc.divide_by_vanishing(ext, dom.k, dom.extended_k))
+    polys = [a, b, orc.gen_scalars(n, seed=95)]
+    sc = orc.gen_scalars(3, seed=96)
+    exp = np.zeros((n, 4), np.uint64)
+    for p, s_ in zip(polys, sc):
+        exp = orc.poly_op("axpy", exp, p, s_, threads=THREADS)
+    assert np.array_equal(h2.poly_lincomb(polys, sc), exp)
+    # lookup multiplicities: a table of n distinct values, two input columns of n rows drawn from it
+    rng = np.random.default_rng(97)
+    idx = [rng.integers(0, n, n), rng.integers(0, n, n)]
+    counts = np.bincount(np.concatenate(idx), minlength=n)
+    want = H.fr_array(list(range(int(counts.max()) + 1)))[counts]
+    assert np.array_equal(ev.lookup_multiplicities(a, [a[i] for i in idx], n), want)
+    # g1_fft at 2^19 points (32 MiB): forward, then inverse with n^-1, gives back the input
+    k = 19
+    g = dev.to_host(dev.generate_bases(1 << k, seed=98))
+    w = pow(F.FR_ROOT_OF_UNITY, 1 << (F.FR_S - k), F.FR_MODULUS)
+    fwd, back = np.zeros_like(g), np.zeros_like(g)
+    nat.check(nat.lib().b200_g1_fft(nat.ptr(g), C.c_uint32(k), nat.ptr(F.fr_to_limbs(w)), None, nat.ptr(fwd)))
+    nat.check(nat.lib().b200_g1_fft(nat.ptr(fwd), C.c_uint32(k), nat.ptr(F.fr_to_limbs(F.fr_inv(w))), nat.ptr(F.fr_to_limbs(F.fr_inv(1 << k))), nat.ptr(back)))
+    assert not np.array_equal(fwd, g) and np.array_equal(back, g)
+    # bases_register from the host (2^19 + 3 points, 32 MiB + 192 B) builds the same table as from the device
+    nb = (1 << 19) + 3
+    d_pts = dev.generate_bases(nb, seed=99)
+    hb, db = h2.Bases(dev.to_host(d_pts)), dev.DeviceBases(d_pts)
+    col = orc.gen_scalars(nb, seed=100)
+    assert np.array_equal(h2.best_multiexp(col, hb), dev.normalize(dev.msm_batch(db, dev.from_host(col)))[0])
+    hb.release()
+    db.release()
+
+
+def test_launch_count_matches_the_profiler():
+    """b200_launch_count against the library's kernels (all named k_*) that torch.profiler sees in the same window: a first-use
+    NTT plan, the empty MSM and lookup calls, and one call of every other operation family."""
+    import re
+
+    import torch
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    from ezkl_b200 import device as dev
+    from ezkl_b200 import evaluation as ev
+    from ezkl_b200 import fields as F
+    L = nat.lib()
+    r = F.FR_MODULUS
+    k = 12
+    n = 1 << k
+    # omega^3 is another primitive 2^k-th root of unity, so no earlier call has built its plan
+    w3 = F.fr_to_limbs(pow(F.FR_ROOT_OF_UNITY, 3 << (F.FR_S - k), r))
+    a, b = orc.gen_scalars(n, seed=110), orc.gen_scalars(n, seed=111)
+    x = orc.gen_scalars(1, seed=112)[0]
+    d_pts = dev.generate_bases(256, seed=113)
+    pts = dev.to_host(d_pts)
+    d_sc = dev.from_host(orc.gen_scalars(256, seed=114))
+    d_xyzz = torch.zeros((2, 16), dtype=torch.int64, device="cuda")
+    dom = h2.EvaluationDomain(5, 10)
+    expr = ev.fold_y([ev.Query(0) * ev.Query(1, 1) - ev.Query(1, -1)], 0x1234)
+    prog = ev.QuotientProgram(expr)
+    polys = [orc.gen_scalars(dom.n, seed=115), orc.gen_scalars(dom.n, seed=116)]
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        l0 = nat.launch_count()
+        fwd = a.copy()
+        nat.check(L.b200_fft(nat.ptr(fwd), C.c_uint32(k), nat.ptr(w3)))                          # plan tables + passes
+        bases, d_bases = h2.Bases(pts), dev.DeviceBases(d_pts)                                     # table builds
+        nat.check(L.b200_msm_batch_dev(C.c_uint64(bases.handle), nat.dev(d_sc.data_ptr()), C.c_size_t(0), C.c_size_t(0), C.c_size_t(2),
+                                       nat.dev(d_xyzz.data_ptr()), dev._stream()))                 # n = 0: a memset only
+        h2.best_multiexp(orc.gen_scalars(256, seed=117), bases)
+        dev.g1_sum(dev.msm_batch(d_bases, d_sc).reshape(1, 1, 16).contiguous())
+        dev.fixed_base_mul(d_sc)
+        dev.generate_bases(16, seed=118)
+        h2.g_to_lagrange(pts[:16], 4)
+        dev.ntt(dev.from_host(a), k, w3)
+        ev.lookup_multiplicities(a[:64], [a[:1]], 0)                                               # n_rows = 0
+        ev.lookup_multiplicities(a[:64], [a[:8]], 8)
+        h2.poly_op("mul", a, b)
+        h2.poly_lincomb([a, b], orc.gen_scalars(2, seed=119))
+        h2.eval_polynomial(a, x)
+        h2.kate_division(a, x)
+        h2.batch_invert(a)
+        h2.prefix_scan(a, x, True)
+        ext = dom.coeff_to_extended_batch(polys)
+        dom.divide_by_vanishing_poly(ev.evaluate_h(prog, ext, dom.k, dom.extended_k))
+        ev.evaluate_h_from_polys(prog, polys, dom, finish=True)
+        torch.cuda.synchronize()
+        launched = nat.launch_count() - l0
+    bases.release()
+    d_bases.release()
+    kernels = [e.name for e in prof.events() if e.device_type == DeviceType.CUDA and re.search(r"(^|[\s:])k_\w", e.name)]
+    assert kernels and launched == len(kernels), (launched, len(kernels), sorted(set(kernels)))
