@@ -3,6 +3,7 @@
 // multi-device host-pointer paths and the host-side tail (point normalisation).  No CPU fallback lives here: every compute
 // entry point needs an initialised CUDA device and fails with an error code otherwise.
 #include <atomic>
+#include <cerrno>
 #include <condition_variable>
 #include <cstdlib>
 #include <cstring>
@@ -37,8 +38,16 @@ int sm_count() {
     return v;
 }
 static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
-static void read_config() {
+static int read_config() {
     Config c;
+    if (const char* e = getenv("B200_MSM_TABLE_MB")) {
+        char* end = nullptr;
+        errno = 0;
+        const unsigned long long mb = strtoull(e, &end, 10);
+        B200_CHECK(*e >= '0' && *e <= '9' && *end == '\0' && errno == 0 && mb >= 1 && mb < ((unsigned long long)1 << 40), -1,
+                   "b200_init: B200_MSM_TABLE_MB = '%s' is not a positive whole number of MiB", e);
+        c.msm_table_budget = (size_t)mb << 20;
+    }
     if (const char* e = getenv("B200_WS_BUDGET_MB")) c.ws_budget_call = (size_t)atol(e) << 20;
     if (const char* e = getenv("B200_WS_TOTAL_MB")) c.ws_budget_total = (size_t)atol(e) << 20;
     c.ntt_v1 = env_int("B200_NTT_V", 2) == 1;
@@ -50,6 +59,7 @@ static void read_config() {
     c.msm_reduce_threads = env_int("B200_MSM_REDUCE_THREADS", 0);
     c.shard_min_logn = env_int("B200_SHARD_MIN_LOGN", 22);
     g_cfg = c;
+    return 0;
 }
 
 // ---- process state ----------------------------------------------------------------------------------------------------------------
@@ -64,7 +74,7 @@ static std::mutex g_mu;                         // tables, plans, context regist
 
 // One registered base vector: a window-precomputed table replica per device of the process.
 struct BaseSet {
-    size_t n = 0; int c = 0, W = 0;
+    size_t n = 0; int c = 0, W = 0, s = 1, L = 0;
     MsmTable* t[MAX_DEV] = {};
 };
 static std::unordered_map<uint64_t, BaseSet*> g_tables;
@@ -419,6 +429,7 @@ static int msm_dev_on(Ctx* c, cudaStream_t st, const BaseSet* bs, const Fr* sc, 
     size_t sub = call_budget() / (per_col ? per_col : 1);
     if (sub < 1) sub = 1;
     if (sub > 4096) sub = 4096;
+    if (sub > (size_t)(65535 / t->s)) sub = 65535 / t->s;          // a reduced table reduces batch * s bucket sets in one grid
     for (size_t b0 = 0; b0 < batch; b0 += sub) {
         const size_t nb = batch - b0 < sub ? batch - b0 : sub;
         if (int rc = msm_run(*t, sc + b0 * stride, n, stride, (int)nb, out + b0, c->msm_ws, st, base_off)) return rc;
@@ -475,10 +486,10 @@ static int init_devices(const int* ids, int n) {
         B200_CHECK(same, -1, "b200_init: already initialised with another device set (call b200_shutdown first)");
         return 0;
     }
+    if (int rc = read_config()) return rc;
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
     if (e != cudaSuccess || count == 0) { set_error("b200_init: no CUDA device (%s)", cudaGetErrorString(e)); return -2; }
-    read_config();
     int first = 0;
     for (int s = 0; s < n; ++s) {
         int device = ids[s];
@@ -600,8 +611,11 @@ int b200_sync_all(void) {
 }
 
 // ---- bases ---------------------------------------------------------------------------------------------------
-static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, size_t n, int window_bits, uint64_t* handle) {
-    B200_CHECK(d_bases && handle && n > 0, -1, "bases_register: null argument or n == 0");
+// The bases come from the device (d_bases, copied into level 0) or from the host (h_bases, uploaded straight into level 0 of the
+// new table, so no staging buffer of the calling thread grows to the size of an SRS vector).  max_table_bytes = 0: the configured budget.
+static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, const b200_g1_affine* h_bases, size_t n, int window_bits, size_t max_table_bytes,
+                             uint64_t* handle) {
+    B200_CHECK((d_bases || h_bases) && handle && n > 0, -1, "bases_register: null argument or n == 0");
     B200_CHECK(window_bits == 0 || (window_bits >= 4 && window_bits <= 24), -1, "bases_register: window_bits %d not in {0, 4..24}", window_bits);
     BaseSet* bs = new BaseSet();
     auto fail = [&](int rc) {
@@ -612,18 +626,22 @@ static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, size_
     };
     MsmTable* t = new MsmTable();
     bs->t[c->slot] = t;
-    if (int rc = msm_table_build(t, reinterpret_cast<const G1Affine*>(d_bases), n, window_bits, st)) return fail(rc);
-    bs->n = n; bs->c = t->c; bs->W = t->W;
+    if (int rc = msm_table_alloc(t, n, window_bits, max_table_bytes ? max_table_bytes : config().msm_table_budget)) return fail(rc);
+    if (h_bases) {
+        if (int rc = h2d_one(c, t->d_table, h_bases, sizeof(G1Affine) * n, st)) return fail(rc);
+    }
+    if (int rc = msm_table_build(t, reinterpret_cast<const G1Affine*>(d_bases), st)) return fail(rc);
+    bs->n = n; bs->c = t->c; bs->W = t->W; bs->s = t->s; bs->L = t->L;
     // replicas: the finished table crosses NVLink once per extra device (cheaper than rebuilding: one inversion per point and level)
     for (int s = 0; s < g_ndev.load(); ++s) if (s != c->slot) {
         MsmTable* r = new MsmTable();
         *r = *t; r->d_table = nullptr; r->device = g_devs[s].id;
         bs->t[s] = r;
         cudaSetDevice(r->device);
-        cudaError_t e = cudaMalloc(&r->d_table, sizeof(G1Affine) * n * t->W);
+        cudaError_t e = cudaMalloc(&r->d_table, t->bytes());
         cudaSetDevice(c->dev);
         if (e != cudaSuccess) { set_error("bases_register: replica on device %d: %s", r->device, cudaGetErrorString(e)); return fail(-2); }
-        e = cudaMemcpyPeerAsync(r->d_table, r->device, t->d_table, t->device, sizeof(G1Affine) * n * t->W, st);
+        e = cudaMemcpyPeerAsync(r->d_table, r->device, t->d_table, t->device, t->bytes(), st);
         if (e != cudaSuccess) { set_error("bases_register: peer copy: %s", cudaGetErrorString(e)); return fail(-2); }
     }
     cudaError_t e = cudaStreamSynchronize(st);
@@ -633,17 +651,21 @@ static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, size_
     g_tables[*handle] = bs;
     return 0;
 }
-int b200_bases_register_dev(const void* d_bases, size_t n, int window_bits, uint64_t* handle) {
+int b200_bases_register_ex_dev(const void* d_bases, size_t n, int window_bits, size_t max_table_bytes, uint64_t* handle) {
     B200_ENTER(c, d_bases); StreamScope ss(c, nullptr);
-    return bases_register_on(c, ss.st, d_bases, n, window_bits, handle);
+    return bases_register_on(c, ss.st, d_bases, nullptr, n, window_bits, max_table_bytes, handle);
 }
-int b200_bases_register(const b200_g1_affine* bases, size_t n, int window_bits, uint64_t* handle) {
+int b200_bases_register_ex(const b200_g1_affine* bases, size_t n, int window_bits, size_t max_table_bytes, uint64_t* handle) {
     B200_ENTER(c, nullptr);
     B200_CHECK(bases && handle && n > 0, -1, "bases_register: null argument or n == 0");
-    if (c->stage_a.ensure(sizeof(G1Affine) * n)) return -2;
     StreamScope ss(c, nullptr);
-    if (int rc = h2d_one(c, c->stage_a.p, bases, sizeof(G1Affine) * n, ss.st)) return rc;
-    return bases_register_on(c, ss.st, c->stage_a.p, n, window_bits, handle);
+    return bases_register_on(c, ss.st, nullptr, bases, n, window_bits, max_table_bytes, handle);
+}
+int b200_bases_register_dev(const void* d_bases, size_t n, int window_bits, uint64_t* handle) {
+    return b200_bases_register_ex_dev(d_bases, n, window_bits, 0, handle);
+}
+int b200_bases_register(const b200_g1_affine* bases, size_t n, int window_bits, uint64_t* handle) {
+    return b200_bases_register_ex(bases, n, window_bits, 0, handle);
 }
 int b200_bases_release(uint64_t handle) {
     CallGuard cg; if (!cg.ok) return -3;
@@ -667,6 +689,14 @@ int b200_bases_info(uint64_t handle, size_t* n, int* window_bits, int* windows) 
     if (n) *n = t->n;
     if (window_bits) *window_bits = t->c;
     if (windows) *windows = t->W;
+    return 0;
+}
+int b200_bases_table(uint64_t handle, int* levels, int* windows_per_level, size_t* table_bytes) {
+    BaseSet* t = find_bases(handle);
+    B200_CHECK(t, -1, "bases_table: unknown handle %llu", (unsigned long long)handle);
+    if (levels) *levels = t->L;
+    if (windows_per_level) *windows_per_level = t->s;
+    if (table_bytes) *table_bytes = sizeof(G1Affine) * t->n * (size_t)t->L;
     return 0;
 }
 

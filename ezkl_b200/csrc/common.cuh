@@ -99,13 +99,15 @@ struct Config {
     int msm_reduce2 = 0;            // B200_MSM_REDUCE2=2: four-lane cooperative reduction tail for <= 3 columns (A/B runs)
     int msm_reduce_threads = 0;     // B200_MSM_REDUCE_THREADS: CTA size of the bucket reduction (32 / 64 / 128 / 256), 0 = automatic
     int shard_min_logn = 22;        // B200_SHARD_MIN_LOGN: a single transform of at least this size is sharded across the devices
+    size_t msm_table_budget = (size_t)16 << 30;   // B200_MSM_TABLE_MB: base-table bytes per registered vector and device (msm_pick_levels)
 };
 const Config& config();
 // Streaming multiprocessors of the current device (132 on an H100 SXM); grids are sized in multiples of it.
 int sm_count();
 
 // Optional device-side timing of kernel classes with CUDA events on the launching stream (bench.py's roofline leg).
-enum ProfClass { PROF_MSM_ACCUMULATE = 0, PROF_MSM_TOTAL = 1, PROF_NTT = 2, PROF_POLY = 3, PROF_MSM_RECODE = 4, PROF_MSM_TAIL = 5, PROF_QUOTIENT = 6, PROF_NCLASS = 7 };
+enum ProfClass { PROF_MSM_ACCUMULATE = 0, PROF_MSM_TOTAL = 1, PROF_NTT = 2, PROF_POLY = 3, PROF_MSM_RECODE = 4, PROF_MSM_TAIL = 5, PROF_QUOTIENT = 6,
+                 PROF_MSM_SCAN = 7, PROF_MSM_REDUCE = 8, PROF_MSM_FOLD = 9, PROF_NCLASS = 10 };
 bool prof_enabled();
 void prof_mark(int cls, cudaStream_t st, bool begin);
 struct ProfScope {

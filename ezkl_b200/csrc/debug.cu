@@ -266,6 +266,30 @@ int b200_debug_digits_host(const b200_fr* s_canonical, size_t n, int c, int32_t*
     }
     return 0;
 }
+// host-only: where each digit of the recoding above goes in a table of `wpl` windows per level (the slot walk k_digits runs):
+// out[(i * W + w) * 4 + {0, 1, 2, 3}] = level, bucket set, bucket (-1 for a zero digit), sign (-1, 0, 1)
+int b200_debug_digit_slots_host(const b200_fr* s_canonical, size_t n, int c, int wpl, int32_t* out) {
+    const int W = (255 + c - 1) / c;
+    for (size_t i = 0; i < n; ++i) {
+        uint32_t v[8]; memcpy(v, &s_canonical[i], 32);
+        uint32_t carry = 0;
+        MsmWindowSlot slot;
+        for (int w = 0; w < W; ++w) {
+            const int32_t d = msm_next_digit(v, c, &carry);
+            int32_t* o = out + ((size_t)i * W + w) * 4;
+            o[0] = (int32_t)slot.level; o[1] = slot.r;
+            o[2] = d ? (int32_t)(slot.set_off + (uint32_t)(d < 0 ? -d : d) - 1u) : -1;
+            o[3] = d < 0 ? -1 : (d > 0 ? 1 : 0);
+            slot.next(c, wpl);
+        }
+    }
+    return 0;
+}
+// host-only: the base-table level policy (msm.cuh)
+int b200_debug_msm_pick_levels(size_t n, int c, size_t max_table_bytes, int* s, int* L) {
+    msm_pick_levels(n, c, max_table_bytes, s, L);
+    return 0;
+}
 // host-only: group law / field code compiled for the CPU through the portable path (not-gpu tests)
 int b200_debug_host_g1_op(int op, const b200_g1_affine* a, const b200_g1_affine* b, b200_g1_affine* out, size_t n) {
     for (size_t i = 0; i < n; ++i) {

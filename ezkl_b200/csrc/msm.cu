@@ -14,6 +14,8 @@
 //   8 k_combine / 9 k_combine_heavy   chunk sums -> bucket sums
 //  10 k_reduce          sum_b (b+1) * B_b by per-thread running sums + small-multiple fix-up + block tree
 //  11 k_final           per-column sum of the block partials -> one XYZZ point per column
+//  12 k_subwindow_fold  only for a reduced table (s > 1 windows per level): 10 and 11 run on the s bucket sets of a column as
+//                       s virtual columns; this Horner chain folds their s results into the column's point
 // HBM traffic per (scalar, base) pair: 32 B scalar (read twice) + W x 64 B table gathers; the kernel is bound by
 // integer issue (IMAD.WIDE), not HBM — see DESIGN.md §kernels.
 #include "msm.cuh"
@@ -46,17 +48,29 @@ __global__ void __launch_bounds__(128) k_table_next_level(const G1Affine* __rest
     next[i] = g1_to_affine(a);
 }
 
-int msm_table_build(MsmTable* t, const G1Affine* d_bases, size_t n, int c, cudaStream_t st) {
+int msm_table_alloc(MsmTable* t, size_t n, int c, size_t max_table_bytes) {
     B200_CHECK(n > 0, -1, "msm_table_build: empty base vector");
     if (c <= 0) c = msm_default_window(n);
-    int W = (255 + c - 1) / c;
-    B200_CHECK((size_t)W * n < ((size_t)1 << 31), -1, "msm_table_build: W*n = %zu exceeds the 31-bit entry index", (size_t)W * n);
-    t->n = n; t->c = c; t->W = W;
+    int W = (255 + c - 1) / c, s = 1, L = W;
+    msm_pick_levels(n, c, max_table_bytes, &s, &L);
+    B200_CHECK((size_t)L * n < ((size_t)1 << 31), -1, "msm_table_build: L*n = %zu exceeds the 31-bit entry index", (size_t)L * n);
+    t->n = n; t->c = c; t->W = W; t->s = s; t->L = L;
     B200_CUDA(cudaGetDevice(&t->device));
-    B200_CUDA(cudaMalloc(&t->d_table, sizeof(G1Affine) * n * W));
-    B200_CUDA(cudaMemcpyAsync(t->d_table, d_bases, sizeof(G1Affine) * n, cudaMemcpyDeviceToDevice, st));
-    for (int w = 1; w < W; ++w) {
-        k_table_next_level<<<div_up(n, 128), 128, 0, st>>>(t->d_table + (size_t)(w - 1) * n, t->d_table + (size_t)w * n, n, c); count_launch();
+    const cudaError_t e = cudaMalloc(&t->d_table, t->bytes());
+    if (e != cudaSuccess) {
+        cudaGetLastError();          // an allocation failure must not surface in a later launch check
+        t->d_table = nullptr;
+        set_error("msm_table_build: %zu MiB table (%d levels of %zu points): %s", t->bytes() >> 20, L, n, cudaGetErrorString(e));
+        return -2;
+    }
+    return 0;
+}
+
+int msm_table_build(MsmTable* t, const G1Affine* d_bases, cudaStream_t st) {
+    const size_t n = t->n;
+    if (d_bases) B200_CUDA(cudaMemcpyAsync(t->d_table, d_bases, sizeof(G1Affine) * n, cudaMemcpyDeviceToDevice, st));
+    for (int j = 1; j < t->L; ++j) {
+        k_table_next_level<<<div_up(n, 128), 128, 0, st>>>(t->d_table + (size_t)(j - 1) * n, t->d_table + (size_t)j * n, n, t->c * t->s); count_launch();
     }
     B200_CUDA(cudaGetLastError());
     return 0;
@@ -67,12 +81,13 @@ void msm_table_free(MsmTable* t) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// 1 / 3: digit extraction, histogram and scatter
-template <bool SCATTER>
+// 1 / 3: digit extraction, histogram and scatter.  SUBWIN (s > 1 windows per table level): window w reads level j = w / s and
+// counts into bucket set r = w % s, i.e. bucket r * 2^(c-1) + |d| - 1; without it j = w, r = 0 (the full table).
+template <bool SCATTER, bool SUBWIN>
 __global__ void __launch_bounds__(256) k_digits(const Fr* __restrict__ scalars, size_t stride, uint32_t n, uint32_t table_n, uint32_t base_off, int c, int W,
                                                  uint32_t nbuckets, uint32_t* __restrict__ counters /*[col][nbuckets]*/,
                                                  const uint32_t* __restrict__ offs /*[col][nbuckets+1]*/, uint32_t* __restrict__ ents, size_t ent_stride,
-                                                 const uint32_t* __restrict__ skew) {
+                                                 const uint32_t* __restrict__ skew, int wpl) {
     const uint32_t col = blockIdx.y;
     const bool aggregate = !SCATTER || skew[col] != 0;        // the counting pass cannot know yet; the scatter pass can
     const Fr* sc = scalars + (size_t)col * stride;
@@ -86,16 +101,18 @@ __global__ void __launch_bounds__(256) k_digits(const Fr* __restrict__ scalars, 
         Fr s = fp_zero<FrTag>();
         if (valid) s = fp_from_mont(fp_load(sc + i));
         uint32_t carry = 0;
+        MsmWindowSlot slot;
 #pragma unroll 1
         for (int w = 0; w < W; ++w) {
             int32_t d = msm_next_digit(s.l, c, &carry);
+            const uint32_t j = SUBWIN ? slot.level : (uint32_t)w;
             const bool nz = d != 0;     // invalid lanes carry s = 0 -> all digits 0
             const unsigned act = __ballot_sync(0xffffffffu, nz);
             if (nz && !aggregate) {
-                const uint32_t bucket = (uint32_t)(d < 0 ? -d : d) - 1u;
-                ent[off[bucket] + atomicAdd(&cnt[bucket], 1u)] = ((uint32_t)w * table_n + base_off + i) | (d < 0 ? 0x80000000u : 0u);
+                const uint32_t bucket = (SUBWIN ? slot.set_off : 0u) + (uint32_t)(d < 0 ? -d : d) - 1u;
+                ent[off[bucket] + atomicAdd(&cnt[bucket], 1u)] = (j * table_n + base_off + i) | (d < 0 ? 0x80000000u : 0u);
             } else if (nz) {
-                const uint32_t bucket = (uint32_t)(d < 0 ? -d : d) - 1u;
+                const uint32_t bucket = (SUBWIN ? slot.set_off : 0u) + (uint32_t)(d < 0 ? -d : d) - 1u;
                 const unsigned peers = __match_any_sync(act, bucket);
                 const int leader = __ffs(peers) - 1;
                 uint32_t base = 0;
@@ -103,9 +120,10 @@ __global__ void __launch_bounds__(256) k_digits(const Fr* __restrict__ scalars, 
                 if (SCATTER) {
                     base = __shfl_sync(peers, base, leader);
                     const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
-                    ent[off[bucket] + base + rank] = ((uint32_t)w * table_n + base_off + i) | (d < 0 ? 0x80000000u : 0u);
+                    ent[off[bucket] + base + rank] = (j * table_n + base_off + i) | (d < 0 ? 0x80000000u : 0u);
                 }
             }
+            if (SUBWIN) slot.next(c, wpl);
         }
     }
 }
@@ -396,6 +414,22 @@ __global__ void __launch_bounds__(TREE_THREADS) k_final_coop(const G1Xyzz* __res
     if (threadIdx.x == 0) out[col] = acc;
 }
 
+// 12 (s > 1 windows per table level): per column, Horner over the s bucket-set results R_r (weight 2^(c*r)):
+//    acc = R_(s-1);  acc = 2^c * acc + R_r for r = s-2 .. 0.   (s-1)*c doublings and s-1 additions per column.
+__global__ void __launch_bounds__(32) k_subwindow_fold(const G1Xyzz* __restrict__ set_sums /*[col][s]*/, int s, int c, uint32_t batch, G1Xyzz* __restrict__ out) {
+    const uint32_t col = blockIdx.x * blockDim.x + threadIdx.x;
+    if (col >= batch) return;
+    const G1Xyzz* rs = set_sums + (size_t)col * s;
+    G1Xyzz acc = rs[s - 1];
+#pragma unroll 1
+    for (int r = s - 2; r >= 0; --r) {
+#pragma unroll 1
+        for (int k = 0; k < c; ++k) acc = g1_dbl(acc);
+        acc = g1_add(acc, rs[r]);
+    }
+    out[col] = acc;
+}
+
 // synthetic distinct bases for benchmarks / tests: out[i] = [h(seed, i)] * G, affine (G = (1, 2))
 __global__ void __launch_bounds__(128) k_g1_generate(uint64_t seed, size_t n, G1Affine* __restrict__ out) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -463,9 +497,9 @@ static uint32_t pick_cap(size_t total_entries) {
 }
 
 size_t msm_workspace_per_column(const MsmTable& t, size_t n) {
-    const size_t nb = (size_t)1 << (t.c - 1), ents = n * t.W;
+    const size_t nb = (size_t)t.s << (t.c - 1), ents = n * t.W;      // s bucket sets per column
     const size_t chunk_stride = nb + ents / 16 + 1;
-    return ents * 4 + chunk_stride * (12 + sizeof(G1Xyzz)) + nb * (sizeof(G1Xyzz) + 24) + 65536;
+    return ents * 4 + chunk_stride * (12 + sizeof(G1Xyzz)) + nb * (sizeof(G1Xyzz) + 24) + 65536 * (size_t)t.s;
 }
 
 int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int batch, G1Xyzz* d_out, MsmWorkspace& ws, cudaStream_t st, size_t base_off) {
@@ -475,8 +509,12 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
         B200_CUDA(cudaMemsetAsync(d_out, 0, sizeof(G1Xyzz) * batch, st));
         return 0;
     }
-    const int c = t.c, W = t.W;
-    const uint32_t nb = 1u << (c - 1);
+    const int c = t.c, W = t.W, s = t.s;
+    B200_CHECK((size_t)batch * s <= 65535, -1, "msm: batch %d x %d bucket sets out of range", batch, s);
+    // s bucket sets of 2^(c-1) per column, laid out [col][r][b]: the same memory as batch * s virtual columns of 2^(c-1) buckets,
+    // which is how the reduction (10, 11) sees them
+    const uint32_t half = 1u << (c - 1), nb = half * (uint32_t)s;
+    const int vcols = batch * s;
     const size_t ent_stride = (size_t)n * W;
     B200_CHECK(ent_stride < ((size_t)1 << 32), -1, "msm: n*W too large");
     const Config& cfg = config();
@@ -494,13 +532,13 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     else if (all_buckets <= ((size_t)1 << 18)) { reduce_m = 8; reduce_threads = 128; }
     else if (all_buckets <= ((size_t)5 << 17)) { reduce_m = 16; reduce_threads = 256; }
     else if (all_buckets < ((size_t)37 << 15)) { reduce_m = 32; reduce_threads = 128; }
-    while (reduce_m > 1 && reduce_m > nb) reduce_m >>= 1;
+    while (reduce_m > 1 && reduce_m > half) reduce_m >>= 1;
     if (cfg.msm_reduce_m >= 1 && cfg.msm_reduce_m <= 4096) reduce_m = (uint32_t)cfg.msm_reduce_m;    // tuning override
     if (cfg.msm_reduce_threads == 32 || cfg.msm_reduce_threads == 64 || cfg.msm_reduce_threads == 128 || cfg.msm_reduce_threads == 256) reduce_threads = (uint32_t)cfg.msm_reduce_threads;
     // the four-lane cooperative tail (ec_coop.cuh) is kept as an opt-in (B200_MSM_REDUCE2=2) for A/B runs
     const bool coop = cfg.msm_reduce2 == 2 && all_buckets <= COOP_MAX_BUCKETS;
     if (coop) { reduce_m = cfg.msm_reduce_m >= 1 ? reduce_m : 8; reduce_threads = TREE_THREADS; }
-    const uint32_t nparts = div_up(div_up(nb, reduce_m), coop ? COOP_LT : reduce_threads);
+    const uint32_t nparts = div_up(div_up(half, reduce_m), coop ? COOP_LT : reduce_threads);
     uint32_t final_threads = 32;
     while (final_threads < (uint32_t)TREE_THREADS && final_threads < nparts) final_threads <<= 1;
 
@@ -526,11 +564,13 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     uint32_t* chunk_start = ws.subs.as<uint32_t>();
     uint32_t* chunk_len = chunk_start + (size_t)batch * chunk_stride;
     uint32_t* order = chunk_len + (size_t)batch * chunk_stride;
-    // sums: chunk_sums | bucket_sums | partials
-    if (ws.sums.ensure(sizeof(G1Xyzz) * ((size_t)batch * chunk_stride + (size_t)batch * nb + (size_t)batch * nparts))) return -2;
+    // sums: chunk_sums | bucket_sums | partials | set_sums (s > 1: one result per bucket set, folded by k_subwindow_fold)
+    const size_t n_set = s > 1 ? (size_t)vcols : 0;
+    if (ws.sums.ensure(sizeof(G1Xyzz) * ((size_t)batch * chunk_stride + (size_t)batch * nb + (size_t)vcols * nparts + n_set))) return -2;
     G1Xyzz* chunk_sums = ws.sums.as<G1Xyzz>();
     G1Xyzz* bucket_sums = chunk_sums + (size_t)batch * chunk_stride;
     G1Xyzz* partials = bucket_sums + (size_t)batch * nb;
+    G1Xyzz* reduced = s > 1 ? partials + (size_t)vcols * nparts : d_out;
 
     ProfScope ps_total(PROF_MSM_TOTAL, st);
     B200_CUDA(cudaMemsetAsync(hist, 0, counts_words * 4, st));
@@ -538,9 +578,16 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     const unsigned sms = (unsigned)sm_count();
     const unsigned dig_blocks = min(div_up(n, 256), sms * 8u);
     dim3 gd(dig_blocks, batch);
-    k_digits<false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr); count_launch();
-    k_scan_buckets<<<batch, 1024, 0, st>>>(hist, offs, chunk_offs, nb, cap, skew); count_launch();
-    k_digits<true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew); count_launch();
+    if (s == 1) k_digits<false, false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr, 1);
+    else k_digits<false, true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr, s);
+    count_launch();
+    {
+        ProfScope ps(PROF_MSM_SCAN, st);
+        k_scan_buckets<<<batch, 1024, 0, st>>>(hist, offs, chunk_offs, nb, cap, skew); count_launch();
+    }
+    if (s == 1) k_digits<true, false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew, 1);
+    else k_digits<true, true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew, s);
+    count_launch();
     k_fill_chunks<<<dim3(div_up(nb, 256), batch), 256, (cap + 1) * 4, st>>>(offs, chunk_offs, nb, cap, chunk_start, chunk_len, chunk_stride, len_hist, heavy, heavy_stride); count_launch();
     k_len_offsets<<<batch, 32, 0, st>>>(len_hist, len_offs, cap); count_launch();
     const unsigned ch_blocks = min(div_up(chunk_stride, 256), sms * 8u);
@@ -554,12 +601,19 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     ProfScope ps_tail(PROF_MSM_TAIL, st);
     k_combine<<<dim3(div_up(nb, 128), batch), 128, 0, st>>>(chunk_offs, nb, chunk_sums, chunk_stride, bucket_sums); count_launch();
     k_combine_heavy<<<dim3(32, batch), TREE_THREADS, 0, st>>>(heavy, heavy_stride, chunk_offs, nb, chunk_sums, chunk_stride, bucket_sums); count_launch();
-    if (coop) {
-        k_reduce_coop<<<dim3(nparts, batch), TREE_THREADS, 0, st>>>(bucket_sums, nb, partials, nparts, reduce_m); count_launch();
-        k_final_coop<<<batch, TREE_THREADS, 0, st>>>(partials, nparts, d_out); count_launch();
-    } else {
-        k_reduce<1><<<dim3(nparts, batch), reduce_threads, 0, st>>>(bucket_sums, nb, partials, nparts, reduce_m); count_launch();
-        k_final<<<batch, final_threads, 0, st>>>(partials, nparts, d_out); count_launch();
+    {
+        ProfScope ps(PROF_MSM_REDUCE, st);
+        if (coop) {
+            k_reduce_coop<<<dim3(nparts, vcols), TREE_THREADS, 0, st>>>(bucket_sums, half, partials, nparts, reduce_m); count_launch();
+            k_final_coop<<<vcols, TREE_THREADS, 0, st>>>(partials, nparts, reduced); count_launch();
+        } else {
+            k_reduce<1><<<dim3(nparts, vcols), reduce_threads, 0, st>>>(bucket_sums, half, partials, nparts, reduce_m); count_launch();
+            k_final<<<vcols, final_threads, 0, st>>>(partials, nparts, reduced); count_launch();
+        }
+    }
+    if (s > 1) {
+        ProfScope ps(PROF_MSM_FOLD, st);
+        k_subwindow_fold<<<div_up((size_t)batch, 32), 32, 0, st>>>(reduced, s, c, (uint32_t)batch, d_out); count_launch();
     }
     B200_CUDA(cudaGetLastError());
     return 0;

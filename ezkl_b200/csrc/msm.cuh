@@ -5,15 +5,20 @@
 
 namespace b200 {
 
-// Device-resident, window-precomputed base table for one SRS vector (ParamsKZG.g or .g_lagrange):
-// level w holds 2^(c*w) * P_i in affine form, so every signed c-bit digit of every scalar lands in ONE shared set of
-// 2^(c-1) buckets and no per-window doubling chain is left for the end.
+// Device-resident, window-precomputed base table for one SRS vector (ParamsKZG.g or .g_lagrange).
+// The W = ceil(255 / c) windows are grouped s to a level; level j holds 2^(c*s*j) * P_i in affine form, L = ceil(W / s) levels.
+// Window w reads level w / s and adds into bucket set w % s (2^(c-1) buckets each); the s set results are folded at the end
+// with (s-1)*c doublings.  s = 1 (the full table) is one shared bucket set and no fold; larger s trades table memory
+// (L * n * 64 B) for an s-fold bucket reduction (msm_pick_levels).
 struct MsmTable {
-    G1Affine* d_table = nullptr;   // [W][n]
+    G1Affine* d_table = nullptr;   // [L][n]
     size_t n = 0;
     int c = 0;
     int W = 0;
+    int s = 1;                     // windows per level (= bucket sets per column)
+    int L = 0;                     // stored levels
     int device = 0;
+    size_t bytes() const { return sizeof(G1Affine) * n * (size_t)L; }
 };
 
 struct MsmWorkspace {
@@ -21,11 +26,25 @@ struct MsmWorkspace {
 };
 
 int msm_default_window(size_t n);
-// Builds the table from n affine points already on the device (copied; caller keeps ownership of d_bases).
-int msm_table_build(MsmTable* t, const G1Affine* d_bases, size_t n, int c, cudaStream_t st);
+// The level policy: the smallest s whose ceil(W / s) * n * 64 B fits max_table_bytes, else s = W (L = 1: the bases alone,
+// whatever the budget).  Pure host function.
+inline void msm_pick_levels(size_t n, int c, size_t max_table_bytes, int* s, int* L) {
+    const int W = (255 + c - 1) / c;
+    const size_t level_bytes = sizeof(G1Affine) * n;
+    for (int k = 1; k <= W; ++k) {
+        const int l = (W + k - 1) / k;
+        if (k == W || (size_t)l * level_bytes <= max_table_bytes) { *s = k; *L = l; return; }
+    }
+}
+// Picks the window (c <= 0: msm_default_window) and the level count, and allocates the table.  Level 0 (the first n points)
+// is left for the caller to fill, e.g. by uploading the bases straight into it.
+int msm_table_alloc(MsmTable* t, size_t n, int c, size_t max_table_bytes);
+// Fills levels 1 .. L-1 from level 0 on `st`.  d_bases != nullptr is first copied into level 0 (caller keeps ownership).
+int msm_table_build(MsmTable* t, const G1Affine* d_bases, cudaStream_t st);
 void msm_table_free(MsmTable* t);
 // out[b] = sum_i scalars[b*stride + i] * P_(base_off + i)   (base_off + n <= table.n), XYZZ form, one point per column, on device.
 // base_off > 0 is the base-split MSM: each device takes a contiguous range of the (scalar, base) pairs against its table replica.
+// batch * t.s must not exceed 65535 (grid.y of the bucket reduction).
 int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int batch, G1Xyzz* d_out,
             MsmWorkspace& ws, cudaStream_t st, size_t base_off = 0);
 int g1_fixed_base_mul_run(const Fr* d_scalars, size_t n, const G1Affine& base, G1Affine* d_out, cudaStream_t st);
@@ -49,5 +68,16 @@ HD int32_t msm_next_digit(uint32_t s[8], int c, uint32_t* carry) {
     *carry = 0;
     return (int32_t)v;
 }
+
+// Where the windows of one scalar go in a table of `wpl` windows per level, low window first: window w reads level w / wpl and
+// counts into bucket set r = w % wpl, whose first bucket is set_off = r * 2^(c-1); a digit d != 0 goes to bucket set_off + |d| - 1.
+struct MsmWindowSlot {
+    uint32_t level = 0, set_off = 0;
+    int r = 0;
+    HD void next(int c, int wpl) {
+        set_off += 1u << (c - 1);
+        if (++r == wpl) { r = 0; set_off = 0; ++level; }
+    }
+};
 
 }  // namespace b200

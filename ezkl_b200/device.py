@@ -92,14 +92,21 @@ def random_scalars(n: int, batch: int | None = None, seed: int = 0, small_bits: 
 
 
 class DeviceBases:
-    def __init__(self, d_points: torch.Tensor, window_bits: int = 0):
+    """Base table built from device points; max_table_bytes as in halo2.Bases (0 = the B200_MSM_TABLE_MB budget)."""
+
+    def __init__(self, d_points: torch.Tensor, window_bits: int = 0, max_table_bytes: int = 0):
         nat.ensure_init()
         _chk(d_points, 8)
         self.n = d_points.shape[0]
         torch.cuda.current_stream().synchronize()
         h = C.c_uint64(0)
-        nat.check(nat.lib().b200_bases_register_dev(nat.dev(d_points.data_ptr()), C.c_size_t(self.n), C.c_int(window_bits), C.byref(h)))
+        nat.check(nat.lib().b200_bases_register_ex_dev(nat.dev(d_points.data_ptr()), C.c_size_t(self.n), C.c_int(window_bits),
+                                                        C.c_size_t(max_table_bytes), C.byref(h)))
         self.handle = h.value
+
+    def info(self) -> dict:
+        from .halo2 import bases_info
+        return bases_info(self.handle)
 
     def release(self):
         if self.handle:

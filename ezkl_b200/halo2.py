@@ -26,35 +26,47 @@ def _fr(a) -> np.ndarray:
 # ------------------------------------------------------------------------------------------------------------
 # SRS bases
 class Bases:
-    """Device-resident, window-precomputed base vector (ParamsKZG.g or .g_lagrange)."""
+    """Device-resident, window-precomputed base vector (ParamsKZG.g or .g_lagrange).
 
-    def __init__(self, points, window_bits: int = 0):
+    max_table_bytes bounds the table on each device (0 = the B200_MSM_TABLE_MB budget, 16 GiB by default): above it the table
+    keeps every s-th window level and the MSM folds s bucket sets at the end.  Results do not depend on it."""
+
+    def __init__(self, points, window_bits: int = 0, max_table_bytes: int = 0):
         nat.ensure_init()
         pts = nat.as_u64(points, 8)
         self.n = pts.shape[0]
         h = C.c_uint64(0)
-        nat.check(nat.lib().b200_bases_register(nat.ptr(pts), C.c_size_t(self.n), C.c_int(window_bits), C.byref(h)))
+        nat.check(nat.lib().b200_bases_register_ex(nat.ptr(pts), C.c_size_t(self.n), C.c_int(window_bits), C.c_size_t(max_table_bytes), C.byref(h)))
         self.handle = h.value
 
     @classmethod
-    def from_device(cls, d_ptr: int, n: int, window_bits: int = 0):
+    def from_device(cls, d_ptr: int, n: int, window_bits: int = 0, max_table_bytes: int = 0):
         nat.ensure_init()
         self = cls.__new__(cls)
         self.n = n
         h = C.c_uint64(0)
-        nat.check(nat.lib().b200_bases_register_dev(nat.dev(d_ptr), C.c_size_t(n), C.c_int(window_bits), C.byref(h)))
+        nat.check(nat.lib().b200_bases_register_ex_dev(nat.dev(d_ptr), C.c_size_t(n), C.c_int(window_bits), C.c_size_t(max_table_bytes), C.byref(h)))
         self.handle = h.value
         return self
 
     def info(self):
-        n, c, w = C.c_size_t(0), C.c_int(0), C.c_int(0)
-        nat.check(nat.lib().b200_bases_info(C.c_uint64(self.handle), C.byref(n), C.byref(c), C.byref(w)))
-        return {"n": n.value, "window_bits": c.value, "windows": w.value}
+        return bases_info(self.handle)
 
     def release(self):
         if self.handle:
             nat.check(nat.lib().b200_bases_release(C.c_uint64(self.handle)))
             self.handle = 0
+
+
+def bases_info(handle: int) -> dict:
+    """A registered base table: n, window_bits, windows (W), levels (L stored levels), windows_per_level (s) and table_bytes
+    (per device)."""
+    n, c, w = C.c_size_t(0), C.c_int(0), C.c_int(0)
+    nat.check(nat.lib().b200_bases_info(C.c_uint64(handle), C.byref(n), C.byref(c), C.byref(w)))
+    lv, wpl, nbytes = C.c_int(0), C.c_int(0), C.c_size_t(0)
+    nat.check(nat.lib().b200_bases_table(C.c_uint64(handle), C.byref(lv), C.byref(wpl), C.byref(nbytes)))
+    return {"n": n.value, "window_bits": c.value, "windows": w.value, "levels": lv.value, "windows_per_level": wpl.value,
+            "table_bytes": nbytes.value}
 
 
 # ------------------------------------------------------------------------------------------------------------

@@ -60,19 +60,36 @@ uint64_t b200_launch_count(void);
 
 /* device-side timing of kernel classes with CUDA events on the launching stream (off by default).
  * cls: 0 = MSM bucket-accumulation kernel, 1 = whole MSM pipeline, 2 = NTT (all passes of a call), 3 = poly, 4 = MSM digit recoding +
- * bucket sort (kernels 1-6), 5 = MSM tail (combine, bucket reduction, final sum), 6 = evaluate_h kernel.
+ * bucket sort (kernels 1-6), 5 = MSM tail (combine, bucket reduction, final sum), 6 = evaluate_h kernel, 7 = MSM bucket scan
+ * (k_scan_buckets), 8 = MSM bucket reduction and final sum, 9 = MSM sub-window fold (reduced tables only).
  * b200_profile_enable(1) clears earlier records; b200_profile_read synchronises the device and sums the class. */
 int b200_profile_enable(int on);
 int b200_profile_read(int cls, double* total_ms, uint64_t* count);
 
 /* ---- SRS bases: ParamsKZG.g / .g_lagrange uploaded once (src/pfsys/srs.rs:30-47 loads them; every commit reuses them).
- *      Registration builds the window-precomputed table on the device.  window_bits = 0 picks it from n.
+ *      Registration builds the window-precomputed table on the device.  window_bits = c (0 picks it from n) splits a scalar into
+ *      W = ceil(255 / c) signed windows.  The table stores L = ceil(W / s) levels, level j = 2^(c*s*j) * P_i (affine, 64 B per
+ *      point), so it takes L * n * 64 B per device.  s = 1 is the full table: every window shares one set of 2^(c-1) buckets.
+ *      s > 1 (a reduced table) gives each of the s windows of a level its own bucket set and folds the s results at the end
+ *      with (s-1)*c doublings: the same bucket additions per scalar, an s-fold bucket reduction.
+ *      Level count: the smallest s whose table fits the budget, and never fewer than one level (the bases themselves), so a
+ *      budget smaller than one level gives L = 1 rather than an error.  The budget is per registered vector and per device:
+ *      max_table_bytes of b200_bases_register_ex[_dev], or, when that is 0 and for b200_bases_register[_dev], the process budget
+ *      B200_MSM_TABLE_MB (MiB, a positive whole number, read in b200_init, which fails with -1 on anything else; default 16384 =
+ *      16 GiB).  At the default window the default budget keeps the full table up to n = 2^24 (13 GiB) and gives s = 2, L = 7
+ *      (14 GiB) at 2^25 and s = 4, L = 4 (16 GiB) at 2^26.  MSM results are normalised, so they are identical for every level count.
+ *      Cost of a reduced table, measured for n = 2^20 .. 2^26 on an H100 80GB HBM3 at 700 W (DESIGN.md §4.2): 289 M pairs/s at 2^26
+ *      and the default budget against 313 M with a 28 GiB table; 297 M against 318 M at 2^24 with half the full table.
  *      A handle may be used from any number of threads at once; b200_bases_release (and b200_shutdown, which releases every
  *      handle) must not run while another thread still has an MSM in flight on that handle (ParamsKZG outlives its commits). */
 int b200_bases_register(const b200_g1_affine* bases, size_t n, int window_bits, uint64_t* handle);
 int b200_bases_register_dev(const void* d_bases, size_t n, int window_bits, uint64_t* handle);
+int b200_bases_register_ex(const b200_g1_affine* bases, size_t n, int window_bits, size_t max_table_bytes, uint64_t* handle);
+int b200_bases_register_ex_dev(const void* d_bases, size_t n, int window_bits, size_t max_table_bytes, uint64_t* handle);
 int b200_bases_release(uint64_t handle);
 int b200_bases_info(uint64_t handle, size_t* n, int* window_bits, int* windows);
+/* the table's layout: stored levels L, windows per level s, bytes per device (L * n * 64) */
+int b200_bases_table(uint64_t handle, int* levels, int* windows_per_level, size_t* table_bytes);
 
 /* ---- MSM: halo2_proofs::arithmetic::best_multiexp / ParamsKZG::{commit, commit_lagrange}
  *      (in-tree caller: /root/reference/src/circuit/modules/polycommit.rs:71).  n <= registered length. */
