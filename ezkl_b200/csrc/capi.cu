@@ -50,12 +50,7 @@ static int read_config() {
     }
     if (const char* e = getenv("B200_WS_BUDGET_MB")) c.ws_budget_call = (size_t)atol(e) << 20;
     if (const char* e = getenv("B200_WS_TOTAL_MB")) c.ws_budget_total = (size_t)atol(e) << 20;
-    c.ntt_v1 = env_int("B200_NTT_V", 2) == 1;
-    c.ntt_logg = env_int("B200_NTT_LOGG", -1);
-    c.ntt_threads = env_int("B200_NTT_THREADS", 0);
-    c.ntt_nofull = getenv("B200_NTT_NOFULL") != nullptr;
     c.msm_reduce_m = env_int("B200_MSM_REDUCE_M", 0);
-    c.msm_reduce2 = env_int("B200_MSM_REDUCE2", 0);
     c.msm_reduce_threads = env_int("B200_MSM_REDUCE_THREADS", 0);
     c.shard_min_logn = env_int("B200_SHARD_MIN_LOGN", 22);
     g_cfg = c;

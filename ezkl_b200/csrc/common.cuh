@@ -91,12 +91,7 @@ struct StagingRing {
 struct Config {
     size_t ws_budget_call = 0;      // B200_WS_BUDGET_MB: fixed per-call scratch budget (tests use it to force the batch-split paths); 0 = derive
     size_t ws_budget_total = (size_t)24 << 30;   // scratch the library may hold across all calling threads of a device (of an 80 GB H100)
-    int ntt_v1 = 0;                 // B200_NTT_V=1: radix-2 shared-memory pass everywhere
-    int ntt_logg = -1;              // B200_NTT_LOGG
-    int ntt_threads = 0;            // B200_NTT_THREADS (v1 pass)
-    int ntt_nofull = 0;             // B200_NTT_NOFULL: two-level inter-pass twiddles even when the full table exists
-    int msm_reduce_m = 0;           // B200_MSM_REDUCE_M
-    int msm_reduce2 = 0;            // B200_MSM_REDUCE2=2: four-lane cooperative reduction tail for <= 3 columns (A/B runs)
+    int msm_reduce_m = 0;           // B200_MSM_REDUCE_M: buckets per thread of the bucket reduction (1..4096), 0 = automatic
     int msm_reduce_threads = 0;     // B200_MSM_REDUCE_THREADS: CTA size of the bucket reduction (32 / 64 / 128 / 256), 0 = automatic
     int shard_min_logn = 22;        // B200_SHARD_MIN_LOGN: a single transform of at least this size is sharded across the devices
     size_t msm_table_budget = (size_t)16 << 30;   // B200_MSM_TABLE_MB: base-table bytes per registered vector and device (msm_pick_levels)

@@ -1,11 +1,7 @@
 // debug.cu — small self-test entry points (b200_debug_*) used only by tests/ to localise a failure to one layer
 // (field arithmetic, group law, digit recoding) before the composite kernels are blamed.  Not part of the drop-in ABI.
 #include "../../include/ezkl_b200.h"
-#include <cfenv>
-#include <vector>
 #include "msm.cuh"
-#include "../../tools/experiments/fd.cuh"
-#include "../../tools/experiments/msm_affine.cuh"
 
 namespace b200 {
 template <class Tag>
@@ -111,31 +107,6 @@ __global__ void __launch_bounds__(256) k_bench_pipe(uint64_t* out, int iters) {
         out[t] = (uint64_t)(c0 + c1 + c2 + c3 + c4 + c5 + c6 + c7);
     }
 }
-// ---- FP64-pipe multiplier (fd.cuh) -----------------------------------------------------------------------------------------
-// out = fd_mul(a, b) re-sliced back to the 256-bit wire container: a * b * 2^-260 mod N, possibly + N (not canonical)
-template <class T>
-__global__ void k_dbg_fd_mul(const Fp<typename T::Wire>* a, const Fp<typename T::Wire>* b, Fp<typename T::Wire>* o, size_t n) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    fp_store(o + i, fd_to_wire(fd_mul(fd_from_wire<T>(fp_load(a + i)), fd_from_wire<T>(fp_load(b + i)))));
-}
-// throughput: DFMA_WARPS of every 8 warps run a chain of FP64-pipe multiplications, the others the integer-pipe chain
-template <int DFMA_WARPS>
-__global__ void __launch_bounds__(256) k_bench_hybrid(Fq* out, int iters) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    Fq x = fp_one<FqTag>(), y = fp_one<FqTag>();
-    x.l[0] ^= t; y.l[1] ^= (t * 2654435761u);
-    if ((int)((threadIdx.x >> 5) & 7) < DFMA_WARPS) {
-        Fd<FdFqTag> u = fd_from_wire<FdFqTag>(x), v = fd_from_wire<FdFqTag>(y);
-#pragma unroll 1
-        for (int i = 0; i < iters; ++i) u = fd_mul(u, v);
-        x = fd_to_wire(u);
-    } else {
-#pragma unroll 1
-        for (int i = 0; i < iters; ++i) x = x * y;
-    }
-    fp_store(out + t, x);
-}
 }  // namespace b200
 using namespace b200;
 
@@ -174,40 +145,6 @@ int b200_debug_digits(const b200_fr* s, size_t n, int c, int32_t* out /* n * cei
     cudaFree(ds); cudaFree(dout);
     return 0;
 }
-int b200_debug_fd_mul(int field, const b200_fr* a, const b200_fr* b, b200_fr* out, size_t n) {
-    void *da, *db, *dout;
-    B200_CUDA(cudaMalloc(&da, 32 * n)); B200_CUDA(cudaMalloc(&db, 32 * n)); B200_CUDA(cudaMalloc(&dout, 32 * n));
-    B200_CUDA(cudaMemcpy(da, a, 32 * n, cudaMemcpyHostToDevice)); B200_CUDA(cudaMemcpy(db, b, 32 * n, cudaMemcpyHostToDevice));
-    if (field == 0) k_dbg_fd_mul<FdFrTag><<<div_up(n, 128), 128>>>((const Fr*)da, (const Fr*)db, (Fr*)dout, n);
-    else k_dbg_fd_mul<FdFqTag><<<div_up(n, 128), 128>>>((const Fq*)da, (const Fq*)db, (Fq*)dout, n);
-    B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaMemcpy(out, dout, 32 * n, cudaMemcpyDeviceToHost));
-    cudaFree(da); cudaFree(db); cudaFree(dout);
-    return 0;
-}
-// host build of the same function (the limb splits are exact in round-toward-zero mode, which this call sets and restores)
-int b200_debug_host_fd_mul(int field, const b200_fr* a, const b200_fr* b, b200_fr* out, size_t n) {
-    const int old = fegetround();
-    fesetround(FE_TOWARDZERO);
-    for (size_t i = 0; i < n; ++i) {
-        if (field == 0) { Fr x, y; memcpy(&x, &a[i], 32); memcpy(&y, &b[i], 32); Fr r = fd_to_wire(fd_mul(fd_from_wire<FdFrTag>(x), fd_from_wire<FdFrTag>(y))); memcpy(&out[i], &r, 32); }
-        else { Fq x, y; memcpy(&x, &a[i], 32); memcpy(&y, &b[i], 32); Fq r = fd_to_wire(fd_mul(fd_from_wire<FdFqTag>(x), fd_from_wire<FdFqTag>(y))); memcpy(&out[i], &r, 32); }
-    }
-    fesetround(old);
-    return 0;
-}
-// CPU run of the batched-affine accumulation bodies (msm_affine.cuh) on host arrays: out[c] = sum of the chunk's points
-int b200_debug_host_affine_chunks(const b200_g1_affine* table, const uint32_t* ents, size_t n_ents, const uint32_t* chunk_start,
-                                  const uint32_t* chunk_len, size_t nchunks, b200_g1_affine* out) {
-    std::vector<b200::G1Affine> tab, res(nchunks);
-    size_t n_pts = 0;
-    for (size_t i = 0; i < n_ents; ++i) if ((ents[i] & 0x7fffffffu) + 1 > n_pts) n_pts = (ents[i] & 0x7fffffffu) + 1;
-    tab.resize(n_pts);
-    memcpy(tab.data(), table, 64 * n_pts);
-    int rc = b200::msm_affine_host_chunks(tab.data(), ents, n_ents, chunk_start, chunk_len, nchunks, res.data());
-    memcpy(out, res.data(), 64 * nchunks);
-    return rc;
-}
 // returns elapsed ms for `iters` operations per thread on blocks x threads threads
 int b200_debug_bench(int variant, int iters, int blocks, int threads, float* ms) {
     Fq* d; B200_CUDA(cudaMalloc(&d, sizeof(Fq) * (size_t)blocks * threads));
@@ -219,15 +156,6 @@ int b200_debug_bench(int variant, int iters, int blocks, int threads, float* ms)
             case 1: k_bench_mul<1><<<blocks, threads>>>(d, iters); break;
             case 2: k_bench_mul<2><<<blocks, threads>>>(d, iters); break;
             case 3: k_bench_mul<3><<<blocks, threads>>>(d, iters); break;
-            case 10: k_bench_hybrid<0><<<blocks, threads>>>(d, iters); break;
-            case 11: k_bench_hybrid<1><<<blocks, threads>>>(d, iters); break;
-            case 12: k_bench_hybrid<2><<<blocks, threads>>>(d, iters); break;
-            case 13: k_bench_hybrid<3><<<blocks, threads>>>(d, iters); break;
-            case 14: k_bench_hybrid<4><<<blocks, threads>>>(d, iters); break;
-            case 15: k_bench_hybrid<5><<<blocks, threads>>>(d, iters); break;
-            case 16: k_bench_hybrid<6><<<blocks, threads>>>(d, iters); break;
-            case 17: k_bench_hybrid<7><<<blocks, threads>>>(d, iters); break;
-            case 18: k_bench_hybrid<8><<<blocks, threads>>>(d, iters); break;
             default: k_bench_mul<4><<<blocks, threads>>>(d, iters); break;
         }
         cudaEventRecord(e1);

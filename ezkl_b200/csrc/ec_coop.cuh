@@ -1,6 +1,7 @@
-// ec_coop.cuh — four-lane cooperative XYZZ addition / doubling for the latency-bound tail of the MSM (bucket reduction, final sums).
+// ec_coop.cuh — four-lane cooperative XYZZ addition / doubling for latency-bound final sums (k_final_coop in msm.cu, behind
+// g1_sum_run: b200_g1_sum_dev and the cross-device combine of b200_msm_sharded_dev).
 //
-// The tail is a chain of ~50-100 DEPENDENT group operations per column with little parallelism (a lone warp pays the
+// A final sum is a chain of DEPENDENT group operations per column with little parallelism (a lone warp pays the
 // latency of its 14 multiplications back to back on every addition, about twice their throughput cost).  Here the four lanes of a quad hold identical copies of the operands and each computes ONE of the independent products
 // of a formula level, the products are exchanged with quad-wide shuffles, and the cheap additions are done redundantly by all four:
 // an addition is 4 multiplication levels deep instead of 14 (doubling: 3 instead of 9), at 14 of 16 (10 of 12) lane-multiplications
@@ -71,18 +72,6 @@ DEV G1Xyzz g1_add_coop4(const G1Xyzz& a, const G1Xyzz& b) {
     o.y = t1 - t2;
     o.zzz = quad_bcast(m, 2, mask);
     return o;
-}
-// k * p for small k, quad-uniform k
-DEV G1Xyzz g1_mul_small_coop4(const G1Xyzz& p, uint32_t k) {
-    G1Xyzz acc = g1_xyzz_identity();
-    int top = 31;
-    while (top > 0 && !((k >> top) & 1)) --top;
-#pragma unroll 1
-    for (int i = top; i >= 0; --i) {
-        acc = g1_dbl_coop4(acc);
-        if ((k >> i) & 1) acc = g1_add_coop4(acc, p);
-    }
-    return acc;
 }
 #endif
 

@@ -6,7 +6,7 @@
 // (un-vendored dependency; call sites /root/reference/src/pfsys/mod.rs:20-22).
 //
 // Device path: generated single-asm-block PTX carry chains (fp_ptx.cuh, validated by fp_gen.py's interpreter).
-// Host path (and -DB200_PORTABLE_FP): portable C++ CIOS, used by the library's own host-side tail
+// Host path: portable C++ CIOS, used by the library's own host-side tail
 // (final point normalisation) and by the host unit tests of the EC formulas.
 #pragma once
 #include <stdint.h>
@@ -62,7 +62,7 @@ struct alignas(16) Fp {
 using Fr = Fp<FrTag>;
 using Fq = Fp<FqTag>;
 
-// ---- portable implementations (host; device when B200_PORTABLE_FP) --------------------------------------
+// ---- portable implementations (host; fp_mul_portable also runs on the device in debug.cu's k_bench_mul<2>) ----------
 template <class Tag>
 HD void fp_mul_portable(uint32_t* r, const uint32_t* a, const uint32_t* b) {
     uint32_t t[10];
@@ -111,7 +111,7 @@ HD void fp_sub_portable(uint32_t* r, const uint32_t* a, const uint32_t* b) {
 
 // ---- dispatch ----------------------------------------------------------------------------------------------
 template <class Tag> struct PtxOps;
-#if defined(__CUDA_ARCH__) && !defined(B200_PORTABLE_FP)
+#if defined(__CUDA_ARCH__)
 template <> struct PtxOps<FrTag> {
     DEV static void mul(uint32_t* r, const uint32_t* a, const uint32_t* b) { fr_mul_ptx(r, a, b); }
     DEV static void add(uint32_t* r, const uint32_t* a, const uint32_t* b) { fr_add_ptx(r, a, b); }
@@ -130,7 +130,7 @@ template <> struct PtxOps<FqTag> {
 
 template <class Tag> HD Fp<Tag> operator*(const Fp<Tag>& a, const Fp<Tag>& b) {
     Fp<Tag> r;
-#if defined(__CUDA_ARCH__) && !defined(B200_PORTABLE_FP)
+#if defined(__CUDA_ARCH__)
     PtxOps<Tag>::mul(r.l, a.l, b.l);
 #else
     fp_mul_portable<Tag>(r.l, a.l, b.l);
@@ -139,7 +139,7 @@ template <class Tag> HD Fp<Tag> operator*(const Fp<Tag>& a, const Fp<Tag>& b) {
 }
 template <class Tag> HD Fp<Tag> operator+(const Fp<Tag>& a, const Fp<Tag>& b) {
     Fp<Tag> r;
-#if defined(__CUDA_ARCH__) && !defined(B200_PORTABLE_FP)
+#if defined(__CUDA_ARCH__)
     PtxOps<Tag>::add(r.l, a.l, b.l);
 #else
     fp_add_portable<Tag>(r.l, a.l, b.l);
@@ -148,16 +148,16 @@ template <class Tag> HD Fp<Tag> operator+(const Fp<Tag>& a, const Fp<Tag>& b) {
 }
 template <class Tag> HD Fp<Tag> operator-(const Fp<Tag>& a, const Fp<Tag>& b) {
     Fp<Tag> r;
-#if defined(__CUDA_ARCH__) && !defined(B200_PORTABLE_FP)
+#if defined(__CUDA_ARCH__)
     PtxOps<Tag>::sub(r.l, a.l, b.l);
 #else
     fp_sub_portable<Tag>(r.l, a.l, b.l);
 #endif
     return r;
 }
-// dedicated squaring on the device (fp_gen.py: gen_sqr, 36 limb products instead of 64); -DB200_NO_SQR falls back to a * a
+// dedicated squaring on the device (fp_gen.py: gen_sqr, 36 limb products instead of 64); the host build computes a * a
 template <class Tag> HD Fp<Tag> fp_sqr(const Fp<Tag>& a) {
-#if defined(__CUDA_ARCH__) && !defined(B200_PORTABLE_FP) && !defined(B200_NO_SQR)
+#if defined(__CUDA_ARCH__)
     Fp<Tag> r;
     PtxOps<Tag>::sqr(r.l, a.l);
     return r;
@@ -192,9 +192,9 @@ template <class Tag> HD bool fp_eq(const Fp<Tag>& a, const Fp<Tag>& b) {
 }
 template <class Tag> HD Fp<Tag> fp_neg(const Fp<Tag>& a) { return fp_zero<Tag>() - a; }
 // a*b + c*d and a*b - c*d with ONE Montgomery reduction on the device (fp_gen.py: gen_mul2, 466 instructions against
-// 312 + 312 + 25); the host build composes them from the single-product operators.  -DB200_NO_MUL2 switches the device back too.
+// 312 + 312 + 25); the host build composes them from the single-product operators.
 template <class Tag> HD Fp<Tag> fp_muladd2(const Fp<Tag>& a, const Fp<Tag>& b, const Fp<Tag>& c, const Fp<Tag>& d) {
-#if defined(__CUDA_ARCH__) && !defined(B200_PORTABLE_FP) && !defined(B200_NO_MUL2)
+#if defined(__CUDA_ARCH__)
     Fp<Tag> r;
     PtxOps<Tag>::mul2(r.l, a.l, b.l, c.l, d.l);
     return r;
@@ -203,7 +203,7 @@ template <class Tag> HD Fp<Tag> fp_muladd2(const Fp<Tag>& a, const Fp<Tag>& b, c
 #endif
 }
 template <class Tag> HD Fp<Tag> fp_mulsub2(const Fp<Tag>& a, const Fp<Tag>& b, const Fp<Tag>& c, const Fp<Tag>& d) {
-#if defined(__CUDA_ARCH__) && !defined(B200_PORTABLE_FP) && !defined(B200_NO_MUL2)
+#if defined(__CUDA_ARCH__)
     return fp_muladd2(a, b, fp_neg(c), d);
 #else
     return a * b - c * d;

@@ -371,9 +371,8 @@ __global__ void __launch_bounds__(TREE_THREADS) k_final(const G1Xyzz* __restrict
     if (threadIdx.x == 0) out[col] = acc;
 }
 
-// ---- four-lane cooperative variants of 10 / 11 (ec_coop.cuh): a quad of lanes is one logical thread, a CTA holds COOP_LT of them ----
+// ---- four-lane cooperative variant of 11 (ec_coop.cuh) for g1_sum_run: a quad of lanes is one logical thread, a CTA holds COOP_LT of them ----
 static constexpr int COOP_LT = TREE_THREADS / 4;
-static constexpr size_t COOP_MAX_BUCKETS = (size_t)3 << 15;
 DEV G1Xyzz block_sum_coop(G1Xyzz v, G1Xyzz* sh) {
     const unsigned lt = threadIdx.x >> 2, q = threadIdx.x & 3;
     if (q == 0) sh[lt] = v;
@@ -384,25 +383,6 @@ DEV G1Xyzz block_sum_coop(G1Xyzz v, G1Xyzz* sh) {
         __syncthreads();
     }
     return v;
-}
-__global__ void __launch_bounds__(TREE_THREADS) k_reduce_coop(const G1Xyzz* __restrict__ bucket_sums, uint32_t nbuckets, G1Xyzz* __restrict__ partials, uint32_t nparts, uint32_t per_thread) {
-    __shared__ G1Xyzz sh[COOP_LT];
-    const uint32_t col = blockIdx.y;
-    const G1Xyzz* bs = bucket_sums + (size_t)col * nbuckets;
-    const uint32_t t = blockIdx.x * COOP_LT + (threadIdx.x >> 2);
-    const uint32_t lo = t * per_thread;
-    G1Xyzz run = g1_xyzz_identity(), acc = g1_xyzz_identity();
-    if (lo < nbuckets) {
-        const uint32_t hi = min(lo + per_thread, nbuckets);
-#pragma unroll 1
-        for (uint32_t b = hi; b-- > lo;) {
-            run = g1_add_coop4(run, bs[b]);
-            acc = g1_add_coop4(acc, run);
-        }
-        if (lo > 0) acc = g1_add_coop4(acc, g1_mul_small_coop4(run, lo));
-    }
-    acc = block_sum_coop(acc, sh);
-    if (threadIdx.x == 0) partials[(size_t)col * nparts + blockIdx.x] = acc;
 }
 __global__ void __launch_bounds__(TREE_THREADS) k_final_coop(const G1Xyzz* __restrict__ partials, uint32_t nparts, G1Xyzz* __restrict__ out) {
     __shared__ G1Xyzz sh[COOP_LT];
@@ -535,10 +515,7 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     while (reduce_m > 1 && reduce_m > half) reduce_m >>= 1;
     if (cfg.msm_reduce_m >= 1 && cfg.msm_reduce_m <= 4096) reduce_m = (uint32_t)cfg.msm_reduce_m;    // tuning override
     if (cfg.msm_reduce_threads == 32 || cfg.msm_reduce_threads == 64 || cfg.msm_reduce_threads == 128 || cfg.msm_reduce_threads == 256) reduce_threads = (uint32_t)cfg.msm_reduce_threads;
-    // the four-lane cooperative tail (ec_coop.cuh) is kept as an opt-in (B200_MSM_REDUCE2=2) for A/B runs
-    const bool coop = cfg.msm_reduce2 == 2 && all_buckets <= COOP_MAX_BUCKETS;
-    if (coop) { reduce_m = cfg.msm_reduce_m >= 1 ? reduce_m : 8; reduce_threads = TREE_THREADS; }
-    const uint32_t nparts = div_up(div_up(half, reduce_m), coop ? COOP_LT : reduce_threads);
+    const uint32_t nparts = div_up(div_up(half, reduce_m), reduce_threads);
     uint32_t final_threads = 32;
     while (final_threads < (uint32_t)TREE_THREADS && final_threads < nparts) final_threads <<= 1;
 
@@ -603,13 +580,8 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     k_combine_heavy<<<dim3(32, batch), TREE_THREADS, 0, st>>>(heavy, heavy_stride, chunk_offs, nb, chunk_sums, chunk_stride, bucket_sums); count_launch();
     {
         ProfScope ps(PROF_MSM_REDUCE, st);
-        if (coop) {
-            k_reduce_coop<<<dim3(nparts, vcols), TREE_THREADS, 0, st>>>(bucket_sums, half, partials, nparts, reduce_m); count_launch();
-            k_final_coop<<<vcols, TREE_THREADS, 0, st>>>(partials, nparts, reduced); count_launch();
-        } else {
-            k_reduce<1><<<dim3(nparts, vcols), reduce_threads, 0, st>>>(bucket_sums, half, partials, nparts, reduce_m); count_launch();
-            k_final<<<vcols, final_threads, 0, st>>>(partials, nparts, reduced); count_launch();
-        }
+        k_reduce<1><<<dim3(nparts, vcols), reduce_threads, 0, st>>>(bucket_sums, half, partials, nparts, reduce_m); count_launch();
+        k_final<<<vcols, final_threads, 0, st>>>(partials, nparts, reduced); count_launch();
     }
     if (s > 1) {
         ProfScope ps(PROF_MSM_FOLD, st);

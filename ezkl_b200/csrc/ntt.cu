@@ -11,7 +11,8 @@
 //     register-resident quad per round, the first round loads global -> registers and the last stores registers -> global
 //     (bit reversal, the inter-pass twiddle omega^(j * i_rest) from a full or two-level table, and the post-scale fused), the
 //     per-stage twiddle table is staged into shared memory with cp.async.bulk (TMA) + mbarrier.
-//   k_ntt_pass (v1): one radix-2 stage per shared-memory round trip; kept for tiny passes and as B200_NTT_V=1.
+//   k_ntt_pass (v1): one radix-2 stage per shared-memory round trip; takes the passes k_ntt_pass2 declines (M < 4, or fewer
+//     than 32 quads per CTA).
 // Coset pre-scaling (zeta^(i mod 3)), zero padding and the 1/N (and zeta^-(i mod 3)) post-scaling of the extended-domain
 // transforms are fused into the first load / last store.  Algorithmic HBM traffic: 64 B per element per transform; this
 // schedule moves 64 B per element per PASS (2 passes up to 2^20, 3 above).  The kernels are bound by the 254-bit multiply
@@ -343,10 +344,8 @@ static int launch_pass_v1(PassArgs& a, uint64_t lines, int batch, cudaStream_t s
 // v2 launch geometry: G lines per CTA chosen so that a CTA holds 1024 elements (256 threads, one quad each; 3 CTAs per SM).
 // Returns false when the pass has to take the v1 kernel (tiny passes).
 static bool plan_pass_v2(PassArgs& a, uint64_t lines, int batch, uint32_t* threads, size_t* smem) {
-    const Config& cfg = config();
-    if (a.logm < 2 || cfg.ntt_v1) return false;
+    if (a.logm < 2) return false;
     uint32_t log_g = a.logm >= 10 ? 0 : 10 - a.logm;
-    if (cfg.ntt_logg >= 0) log_g = (uint32_t)cfg.ntt_logg;
     const uint64_t min_ctas = 2 * (uint64_t)sm_count();
     while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < min_ctas)) --log_g;
     while (log_g > 0 && (a.logm + log_g > 10)) --log_g;
@@ -369,17 +368,14 @@ static int launch_pass(PassArgs& a, uint64_t lines, int batch, cudaStream_t st) 
 
 static int launch_pass_v1(PassArgs& a, uint64_t lines, int batch, cudaStream_t st) {
     // lines per CTA: largest G in {4,2,1} that still yields >= 2 CTAs per SM (and fits shared memory)
-    const Config& cfg = config();
     uint32_t log_g = 2;
     const uint64_t min_ctas = 2 * (uint64_t)sm_count();
     while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < min_ctas)) --log_g;
     while (log_g > 0 && (((size_t)1 << (a.logm + log_g)) + ((size_t)1 << a.logm) / 2) * 32 > 200 * 1024) --log_g;
-    if (cfg.ntt_logg >= 0) { uint32_t v = (uint32_t)cfg.ntt_logg; while (v > 0 && (1u << v) > a.inner_cnt) --v; log_g = v; }
     a.log_g = log_g;
     const size_t smem = (((size_t)1 << (a.logm + log_g)) + (((size_t)1 << a.logm) >> 1)) * 32;
     const uint32_t nbf = (1u << (a.logm + log_g)) >> 1;
-    uint32_t threads = nbf < 32 ? 32 : (nbf > 1024 ? 1024 : nbf);
-    if (cfg.ntt_threads >= 32 && cfg.ntt_threads <= 1024 && (uint32_t)cfg.ntt_threads < threads) threads = (uint32_t)cfg.ntt_threads;
+    const uint32_t threads = nbf < 32 ? 32 : (nbf > 1024 ? 1024 : nbf);
     B200_CUDA(cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     // per device, idempotent
     dim3 grid((unsigned)(lines >> log_g), (unsigned)batch);
     k_ntt_pass<<<grid, threads, smem, st>>>(a); count_launch();
@@ -392,7 +388,7 @@ static int launch_pass_v1(PassArgs& a, uint64_t lines, int batch, cudaStream_t s
 struct PassRole { int in_buf, out_buf; uint64_t lines; };
 static PassRole fill_pass(const NttPlan* p, int idx, uint64_t n_in, PassArgs& a) {
     const uint64_t N1 = 1ull << p->logm[0], N2 = 1ull << p->logm[1], N3 = 1ull << p->logm[2], N23 = N2 * N3;
-    a.t_lo = p->d_lo; a.t_hi = p->d_hi; a.lo_bits = p->lo_bits; a.t_full = config().ntt_nofull ? nullptr : p->d_full;
+    a.t_lo = p->d_lo; a.t_hi = p->d_hi; a.lo_bits = p->lo_bits; a.t_full = p->d_full;
     a.tw_m = p->d_tw[idx]; a.tw_staged = p->d_staged[idx]; a.logm = p->logm[idx];
     a.in_outer_s = a.out_outer_s = 0; a.tw_on = 0; a.rest_is_inner = 0; a.tw_mul = 0;
     PassRole r{0, 2, 1};

@@ -180,60 +180,6 @@ def test_bench_reference_arm_prints_contract_json():
     assert line["e2e"]["h2d_bytes_per_step"] == 0 and "workload" in line["config"]
 
 
-def test_fp64_pipe_multiplier_vs_bigint():
-    """fd.cuh host build: the 5 x 52-bit-limb Montgomery multiplication whose limb products are split with round-toward-zero
-    FMAs must return a * b * 2^-260 mod N (< 2N, limbs normalised) for both fields, including the extremes of the container."""
-    D = nat.dbg_lib()
-    rng = random.Random(3)
-    for fid, N in ((0, pyref.R), (1, pyref.P)):
-        xs = [rng.getrandbits(256) for _ in range(500)] + [0, 1, N - 1, (1 << 256) - 1, N, 2 * N - 1]
-        ys = [rng.getrandbits(256) for _ in range(500)] + [N - 1, (1 << 256) - 1, N - 1, (1 << 256) - 1, N, 2 * N - 1]
-        a = np.stack([H.int_to_limbs(x) for x in xs])
-        b = np.stack([H.int_to_limbs(y) for y in ys])
-        out = np.zeros_like(a)
-        assert D.b200_debug_host_fd_mul(C.c_int(fid), nat.ptr(a), nat.ptr(b), nat.ptr(out), C.c_size_t(len(xs))) == 0
-        rinv = pow(1 << 260, -1, N)
-        for i, (x, y) in enumerate(zip(xs, ys)):
-            v = H.limbs_to_int(out[i])
-            assert v % N == x * y * rinv % N and v < 2 * N, (fid, i)
-
-
-def test_batched_affine_accumulation_bodies_on_host():
-    """tools/experiments/msm_affine.cuh (the batched-affine accumulation EXPERIMENT, not in the product library) run on the CPU: every chunk's tree of batched-affine additions (hierarchical Montgomery trick) must equal
-    the plain sum of its points — incl. repeated points (doubling), P + (-P), identity entries, negated entries, length-1 chunks."""
-    L = nat.lib()
-    rng = random.Random(8)
-    npts = 300
-    table = orc.gen_bases(npts, seed=77, threads=2)
-    table[5] = 0                                            # an identity table entry
-    ents, starts, lens = [], [], []
-    shapes = [1, 2, 3, 4, 5, 7, 8, 16, 31, 33, 64, 100, 1, 2] + [rng.randrange(1, 40) for _ in range(80)]
-    for ln in shapes:
-        starts.append(len(ents))
-        lens.append(ln)
-        for _ in range(ln):
-            ents.append(rng.randrange(npts) | (0x80000000 if rng.random() < 0.3 else 0))
-    # crafted chunks: P + P, P + (-P), identity + P, P + P + P + P
-    for special in ([7, 7], [9, 9 | 0x80000000], [5, 11], [13, 13, 13, 13], [5, 5], [20, 20 | 0x80000000, 21]):
-        starts.append(len(ents))
-        lens.append(len(special))
-        ents.extend(special)
-    ents = np.array(ents, dtype=np.uint32)
-    starts = np.array(starts, dtype=np.uint32)
-    lens = np.array(lens, dtype=np.uint32)
-    out = np.zeros((len(lens), 8), np.uint64)
-    assert nat.dbg_lib().b200_debug_host_affine_chunks(nat.ptr(table), ents.ctypes.data_as(C.c_void_p), C.c_size_t(len(ents)), starts.ctypes.data_as(C.c_void_p),
-                                           lens.ctypes.data_as(C.c_void_p), C.c_size_t(len(lens)), nat.ptr(out)) == 0
-    for c in range(len(lens)):
-        acc = None
-        for e in ents[starts[c]:starts[c] + lens[c]]:
-            p = H.g1_unwire(table[int(e) & 0x7FFFFFFF])
-            if int(e) >> 31:
-                p = pyref.g1_neg(p)
-            acc = pyref.g1_add(acc, p)
-        assert H.g1_unwire(out[c]) == acc, (c, int(lens[c]))
-
-
 def test_generated_field_arithmetic_is_verified_and_current(tmp_path):
     """fp_gen.py executes every emitted PTX instruction list (multiply, add, sub, two-product multiply, squaring) in its own
     interpreter against bigints; the committed fp_ptx.cuh must be exactly what the generator emits today."""

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""NTT throughput sweep on the GPU box (device-resident, CUDA events): G elts/s per (log_n, batch, launch config)."""
+"""NTT throughput sweep on the GPU box (device-resident, CUDA events): G elts/s per (log_n, batch)."""
 import os
 import sys
 
@@ -36,8 +36,6 @@ def run(log_n, batch, reps=5):
 
 if __name__ == "__main__":
     nat.init(0)
-    configs = [("default", {})]          # the library reads its B200_NTT_* overrides once, in b200_init: set them in the environment before launching
     for log_n, batch in ((17, 32), (19, 16), (20, 8), (20, 32), (22, 2), (23, 2), (25, 1)):
-        for name, env in configs:
-            g, ms = run(log_n, batch)
-            print("log_n=%2d batch=%3d  %-18s %8.3f ms  %7.3f G elts/s  (%5.1f GB/s algorithmic)" % (log_n, batch, name, ms, g, g * 64), flush=True)
+        g, ms = run(log_n, batch)
+        print("log_n=%2d batch=%3d  %8.3f ms  %7.3f G elts/s  (%5.1f GB/s algorithmic)" % (log_n, batch, ms, g, g * 64), flush=True)
