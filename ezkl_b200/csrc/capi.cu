@@ -847,6 +847,7 @@ int b200_ntt_dev(const void* d_src, size_t src_stride, size_t n_in, void* d_tmp,
     B200_CHECK(d_src && d_tmp && d_dst && omega, -1, "ntt: null pointer");
     NttScale a, b;
     if (int rc = ntt_scales(pre_mode, pre, post_mode, post, &a, &b)) return rc;
+    B200_CHECK(batch <= 65535, -1, "ntt: batch %zu out of range [0, 65535]", batch);     // before it narrows to the grid's int
     if (batch == 0) return 0;
     StreamScope ss(c, stream);
     return ntt_call(c, ss.st, reinterpret_cast<const Fr*>(d_src), src_stride, n_in, reinterpret_cast<Fr*>(d_tmp), reinterpret_cast<Fr*>(d_dst), dst_stride,

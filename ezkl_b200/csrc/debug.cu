@@ -2,6 +2,7 @@
 // (field arithmetic, group law, digit recoding) before the composite kernels are blamed.  Not part of the drop-in ABI.
 #include "../../include/ezkl_b200.h"
 #include "msm.cuh"
+#include "ntt.cuh"
 
 namespace b200 {
 template <class Tag>
@@ -217,6 +218,22 @@ int b200_debug_digit_slots_host(const b200_fr* s_canonical, size_t n, int c, int
 int b200_debug_msm_pick_levels(size_t n, int c, size_t max_table_bytes, int* s, int* L) {
     msm_pick_levels(n, c, max_table_bytes, s, L);
     return 0;
+}
+// host-only: the NTT pass geometry (ntt.cuh) of a 2^log_n transform of `batch` polynomials on a device of `sm_count` SMs.
+// out[pass * 7 + {0..6}] = kernel (1: k_ntt_pass, 2: k_ntt_pass2), logm, log_g, threads, dynamic shared memory bytes, grid.x,
+// inter-pass twiddle (0: none, the last pass; 1: full omega^e table; 2: two-level t_lo / t_hi tables).  Returns the pass count.
+int b200_debug_ntt_plan_host(uint32_t log_n, int batch, int sm_count, int64_t* out /* 3 * 7 */) {
+    if (log_n < 1 || log_n > 28 || batch < 1 || batch > 65535 || sm_count < 1) return -1;
+    int npass, logm[3];
+    ntt_choose_passes(log_n, &npass, logm);
+    for (int i = 0; i < npass; ++i) {
+        const NttPassShape sh = ntt_pass_shape(npass, logm, i);
+        const NttPassGeom g = ntt_pass_geometry((uint32_t)logm[i], sh.inner_cnt, sh.lines, batch, sm_count);
+        int64_t* o = out + 7 * i;
+        o[0] = g.kernel; o[1] = logm[i]; o[2] = g.log_g; o[3] = g.threads; o[4] = (int64_t)g.smem; o[5] = (int64_t)g.grid_x;
+        o[6] = i == npass - 1 ? 0 : (g.kernel == 2 && ntt_full_table(log_n, npass) ? 1 : 2);     // k_ntt_pass reads t_lo / t_hi only
+    }
+    return npass;
 }
 // host-only: group law / field code compiled for the CPU through the portable path (not-gpu tests)
 int b200_debug_host_g1_op(int op, const b200_g1_affine* a, const b200_g1_affine* b, b200_g1_affine* out, size_t n) {

@@ -35,6 +35,7 @@ struct PassArgs {
     const uint4* tw_staged;      // v2: per-stage twiddles, planar [2][M] (lo plane, hi plane), stage s at offset 2^s - 1
     const Fr* t_full;            // v2: omega^e for every e < N (single-multiply inter-pass twiddle), or null
     NttScale pre, post;
+    uint32_t pre_c0_is_one;      // cyclic pre-scale with c[0] == 1: elements i = 0 mod 3 skip their multiply
     // sharded transform (one polynomial split across devices in contiguous natural-order slices of 2^log_slice elements):
     // element idx of the distributed source / destination lives at peers[idx >> log_slice][idx & (2^log_slice - 1)], reached by
     // ordinary loads / stores on peer-mapped pointers (NVLink), so the exchange steps of the six-step scheme are fused into the passes
@@ -77,7 +78,7 @@ __global__ void __launch_bounds__(1024, 1) k_ntt_pass(const PassArgs a) {
             v = fp_load(src + idx);
             if (a.first) {
                 if (a.pre.mode == 1) v = v * a.pre.c[0];
-                else if (a.pre.mode == 3) { uint32_t m3 = (uint32_t)(idx % 3); if (m3) v = v * a.pre.c[m3]; }
+                else if (a.pre.mode == 3) { uint32_t m3 = (uint32_t)(idx % 3); if (m3 || !a.pre_c0_is_one) v = v * a.pre.c[m3]; }
             }
         }
         sh_put(dlo, dhi, (g << a.logm) + r, v);
@@ -194,7 +195,7 @@ __global__ void __launch_bounds__(256, 3) k_ntt_pass2(const PassArgs a) {
                     x[j] = fp_load(a.peer_on ? a.src_peers[idx >> a.log_slice] + (idx & slice_mask) : src + idx);
                     if (a.first) {
                         if (a.pre.mode == 1) x[j] = x[j] * a.pre.c[0];
-                        else if (a.pre.mode == 3) { uint32_t m3 = (uint32_t)(idx % 3); if (m3) x[j] = x[j] * a.pre.c[m3]; }
+                        else if (a.pre.mode == 3) { uint32_t m3 = (uint32_t)(idx % 3); if (m3 || !a.pre_c0_is_one) x[j] = x[j] * a.pre.c[m3]; }
                     }
                 }
             }
@@ -287,21 +288,13 @@ __global__ void k_powers(Fr base, uint32_t count, Fr* __restrict__ out) {
     if (i < count) fp_store(out + i, fp_pow_u64(base, (uint64_t)i));
 }
 
-static void choose_passes(uint32_t log_n, int* npass, int logm[3]) {
-    logm[0] = logm[1] = logm[2] = 0;
-    if (log_n <= 10) { *npass = 1; logm[0] = (int)log_n; return; }
-    if (log_n <= 20) { *npass = 2; logm[0] = (int)(log_n + 1) / 2; logm[1] = (int)log_n - logm[0]; return; }
-    *npass = 3;
-    logm[0] = (int)(log_n + 2) / 3; logm[1] = (int)(log_n - logm[0] + 1) / 2; logm[2] = (int)log_n - logm[0] - logm[1];
-}
-
 static Fr host_pow(const Fr& b, uint64_t e) { return fp_pow_u64(b, e); }
 
 NttPlan* NttContext::get(uint32_t log_n, const Fr& omega, cudaStream_t st) {
     for (NttPlan* p : plans) if (p->log_n == log_n && fp_eq(p->omega, omega)) return p;
     NttPlan* p = new NttPlan();
     p->log_n = log_n; p->omega = omega;
-    choose_passes(log_n, &p->npass, p->logm);
+    ntt_choose_passes(log_n, &p->npass, p->logm);
     const uint64_t N = 1ull << log_n;
     for (int i = 0; i < p->npass; ++i) {
         const uint32_t M = 1u << p->logm[i], cnt = M > 1 ? M / 2 : 1;
@@ -318,7 +311,7 @@ NttPlan* NttContext::get(uint32_t log_n, const Fr& omega, cudaStream_t st) {
         if (cudaMalloc(&p->d_staged[i], sizeof(uint4) * 2 * M) != cudaSuccess) { set_error("ntt plan: cudaMalloc failed"); delete p; return nullptr; }
         k_stage_twiddles<<<div_up(M, 128), 128, 0, st>>>(host_pow(omega, N / M), (uint32_t)p->logm[i], p->d_staged[i]); count_launch();
     }
-    if (p->npass > 1 && log_n <= 25) {        // full single-multiply twiddle table (N * 32 B; falls back to the two-level table if it does not fit)
+    if (ntt_full_table(log_n, p->npass)) {        // full single-multiply twiddle table (N * 32 B; falls back to the two-level table if it does not fit)
         if (cudaMalloc(&p->d_full, sizeof(Fr) * N) != cudaSuccess) { cudaGetLastError(); p->d_full = nullptr; }
         else { k_powers_run<<<div_up(div_up(N, 32), 128), 128, 0, st>>>(omega, N, p->d_full); count_launch(); }
     }
@@ -339,49 +332,24 @@ void NttContext::release() {
     plans.clear();
 }
 
-static int launch_pass_v1(PassArgs& a, uint64_t lines, int batch, cudaStream_t st);
-
-// v2 launch geometry: G lines per CTA chosen so that a CTA holds 1024 elements (256 threads, one quad each; 3 CTAs per SM).
-// Returns false when the pass has to take the v1 kernel (tiny passes).
-static bool plan_pass_v2(PassArgs& a, uint64_t lines, int batch, uint32_t* threads, size_t* smem) {
-    if (a.logm < 2) return false;
-    uint32_t log_g = a.logm >= 10 ? 0 : 10 - a.logm;
-    const uint64_t min_ctas = 2 * (uint64_t)sm_count();
-    while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < min_ctas)) --log_g;
-    while (log_g > 0 && (a.logm + log_g > 10)) --log_g;
-    if (a.logm + log_g < 7) return false;       // fewer than 32 quads: not worth a CTA
-    a.log_g = log_g;
-    *threads = 1u << (a.logm + log_g - 2);
-    *smem = (((size_t)1 << (a.logm + log_g)) + ((size_t)1 << a.logm)) * 32;
-    return true;
-}
+// one pass on the geometry ntt_pass_geometry (ntt.cuh) picks for this device
 static int launch_pass(PassArgs& a, uint64_t lines, int batch, cudaStream_t st) {
-    uint32_t threads; size_t smem;
-    if (!plan_pass_v2(a, lines, batch, &threads, &smem)) return launch_pass_v1(a, lines, batch, st);
-    B200_CHECK(threads <= 256 && smem <= 200 * 1024, -1, "ntt: pass of 2^%u does not fit a CTA", a.logm);
-    B200_CUDA(cudaFuncSetAttribute(k_ntt_pass2, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     // per device, idempotent
-    dim3 grid((unsigned)(lines >> a.log_g), (unsigned)batch);
-    k_ntt_pass2<<<grid, threads, smem, st>>>(a); count_launch();
+    const NttPassGeom g = ntt_pass_geometry(a.logm, a.inner_cnt, lines, batch, sm_count());
+    a.log_g = g.log_g;
+    const dim3 grid((unsigned)g.grid_x, (unsigned)batch);
+    if (g.kernel == 2) {
+        B200_CHECK(g.threads <= 256 && g.smem <= 200 * 1024, -1, "ntt: pass of 2^%u does not fit a CTA", a.logm);
+        B200_CUDA(cudaFuncSetAttribute(k_ntt_pass2, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     // per device, idempotent
+        k_ntt_pass2<<<grid, g.threads, g.smem, st>>>(a); count_launch();
+    } else {
+        B200_CUDA(cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));      // per device, idempotent
+        k_ntt_pass<<<grid, g.threads, g.smem, st>>>(a); count_launch();
+    }
     B200_CUDA(cudaGetLastError());
     return 0;
 }
 
-static int launch_pass_v1(PassArgs& a, uint64_t lines, int batch, cudaStream_t st) {
-    // lines per CTA: largest G in {4,2,1} that still yields >= 2 CTAs per SM (and fits shared memory)
-    uint32_t log_g = 2;
-    const uint64_t min_ctas = 2 * (uint64_t)sm_count();
-    while (log_g > 0 && ((1u << log_g) > a.inner_cnt || (lines >> log_g) * (uint64_t)batch < min_ctas)) --log_g;
-    while (log_g > 0 && (((size_t)1 << (a.logm + log_g)) + ((size_t)1 << a.logm) / 2) * 32 > 200 * 1024) --log_g;
-    a.log_g = log_g;
-    const size_t smem = (((size_t)1 << (a.logm + log_g)) + (((size_t)1 << a.logm) >> 1)) * 32;
-    const uint32_t nbf = (1u << (a.logm + log_g)) >> 1;
-    const uint32_t threads = nbf < 32 ? 32 : (nbf > 1024 ? 1024 : nbf);
-    B200_CUDA(cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));     // per device, idempotent
-    dim3 grid((unsigned)(lines >> log_g), (unsigned)batch);
-    k_ntt_pass<<<grid, threads, smem, st>>>(a); count_launch();
-    B200_CUDA(cudaGetLastError());
-    return 0;
-}
+static uint32_t pre_c0_is_one(const NttScale& pre) { return pre.mode == 3 && fp_eq(pre.c[0], fp_one<FrTag>()); }
 
 // Geometry of pass `idx` of a plan: which buffer it reads / writes (0 = source, 1 = scratch, 2 = destination), its strides,
 // inter-pass twiddle and how many lines it transforms.  Shared by the single-device and the sharded drivers.
@@ -391,35 +359,37 @@ static PassRole fill_pass(const NttPlan* p, int idx, uint64_t n_in, PassArgs& a)
     a.t_lo = p->d_lo; a.t_hi = p->d_hi; a.lo_bits = p->lo_bits; a.t_full = p->d_full;
     a.tw_m = p->d_tw[idx]; a.tw_staged = p->d_staged[idx]; a.logm = p->logm[idx];
     a.in_outer_s = a.out_outer_s = 0; a.tw_on = 0; a.rest_is_inner = 0; a.tw_mul = 0;
-    PassRole r{0, 2, 1};
+    const NttPassShape sh = ntt_pass_shape(p->npass, p->logm, idx);     // inner_cnt and lines: the same numbers the geometry is chosen from
+    a.inner_cnt = sh.inner_cnt;
+    PassRole r{0, 2, sh.lines};
     if (p->npass == 1) {
-        a.inner_cnt = 1; a.in_r_fast = 1; a.in_rs = 1; a.in_inner_s = 0; a.out_rs = 1; a.out_inner_s = 0; a.n_in = n_in; a.first = a.last = 1;
+        a.in_r_fast = 1; a.in_rs = 1; a.in_inner_s = 0; a.out_rs = 1; a.out_inner_s = 0; a.n_in = n_in; a.first = a.last = 1;
         return r;
     }
     if (p->npass == 2) {
         if (idx == 0) {      // columns i2 (stride 1), transform over i1 (stride N2); twiddle omega^(j1 * i2)
-            a.inner_cnt = (uint32_t)N2; a.in_r_fast = 0; a.in_rs = N2; a.in_inner_s = 1; a.out_rs = N2; a.out_inner_s = 1; a.n_in = n_in; a.first = 1; a.last = 0;
+            a.in_r_fast = 0; a.in_rs = N2; a.in_inner_s = 1; a.out_rs = N2; a.out_inner_s = 1; a.n_in = n_in; a.first = 1; a.last = 0;
             a.tw_on = 1; a.rest_is_inner = 1; a.tw_mul = 1;
-            r = PassRole{0, 1, N2};
+            r.in_buf = 0; r.out_buf = 1;
         } else {             // rows j1 (stride N2), transform over i2 (stride 1); X[j1 + N1*j2]
-            a.inner_cnt = (uint32_t)N1; a.in_r_fast = 1; a.in_rs = 1; a.in_inner_s = N2; a.out_rs = N1; a.out_inner_s = 1; a.n_in = ~0ull; a.first = 0; a.last = 1;
-            r = PassRole{1, 2, N1};
+            a.in_r_fast = 1; a.in_rs = 1; a.in_inner_s = N2; a.out_rs = N1; a.out_inner_s = 1; a.n_in = ~0ull; a.first = 0; a.last = 1;
+            r.in_buf = 1; r.out_buf = 2;
         }
         return r;
     }
     // three passes: i = i1*N2*N3 + i2*N3 + i3  ->  j = j1 + N1*j2 + N1*N2*j3
     if (idx == 0) {
-        a.inner_cnt = (uint32_t)N23; a.in_r_fast = 0; a.in_rs = N23; a.in_inner_s = 1; a.out_rs = N23; a.out_inner_s = 1; a.n_in = n_in; a.first = 1; a.last = 0;
+        a.in_r_fast = 0; a.in_rs = N23; a.in_inner_s = 1; a.out_rs = N23; a.out_inner_s = 1; a.n_in = n_in; a.first = 1; a.last = 0;
         a.tw_on = 1; a.rest_is_inner = 1; a.tw_mul = 1;
-        r = PassRole{0, 1, N23};
+        r.in_buf = 0; r.out_buf = 1;
     } else if (idx == 1) {   // in place on scratch: outer j1 (stride N23), inner i3 (stride 1), transform over i2 (stride N3); twiddle omega^(N1*j2*i3)
-        a.inner_cnt = (uint32_t)N3; a.in_r_fast = 0; a.in_rs = N3; a.in_inner_s = 1; a.in_outer_s = N23; a.out_rs = N3; a.out_inner_s = 1; a.out_outer_s = N23;
+        a.in_r_fast = 0; a.in_rs = N3; a.in_inner_s = 1; a.in_outer_s = N23; a.out_rs = N3; a.out_inner_s = 1; a.out_outer_s = N23;
         a.n_in = ~0ull; a.first = 0; a.last = 0; a.tw_on = 1; a.rest_is_inner = 1; a.tw_mul = N1;
-        r = PassRole{1, 1, N1 * N3};
+        r.in_buf = 1; r.out_buf = 1;
     } else {                 // outer j2 (stride N3), inner j1 (stride N23), transform over i3 (stride 1)
-        a.inner_cnt = (uint32_t)N1; a.in_r_fast = 1; a.in_rs = 1; a.in_inner_s = N23; a.in_outer_s = N3; a.out_rs = N1 * N2; a.out_inner_s = 1; a.out_outer_s = N1;
+        a.in_r_fast = 1; a.in_rs = 1; a.in_inner_s = N23; a.in_outer_s = N3; a.out_rs = N1 * N2; a.out_inner_s = 1; a.out_outer_s = N1;
         a.n_in = ~0ull; a.first = 0; a.last = 1;
-        r = PassRole{1, 2, N1 * N2};
+        r.in_buf = 1; r.out_buf = 2;
     }
     return r;
 }
@@ -430,11 +400,14 @@ int ntt_run(NttPlan* p, const Fr* d_src, size_t src_stride, size_t n_in, Fr* d_t
     B200_CHECK(batch > 0 && batch <= 65535, -1, "ntt: batch %d out of range", batch);
     const uint64_t N = 1ull << log_n;
     B200_CHECK(n_in <= N, -1, "ntt: n_in %zu > N", n_in);
+    B200_CHECK(batch == 1 || (src_stride >= n_in && tmp_stride >= N && dst_stride >= N), -1,
+               "ntt: strides (src %zu, tmp %zu, dst %zu) overlap the polynomials of a batch (n_in %zu, N %llu)", src_stride, tmp_stride, dst_stride,
+               n_in, (unsigned long long)N);
     B200_CHECK(p && p->log_n == log_n && fp_eq(p->omega, omega), -1, "ntt: plan does not match (log_n, omega)");
     ProfScope ps(PROF_NTT, st);
     PassArgs a;
     memset(&a, 0, sizeof a);
-    a.pre = pre; a.post = post;
+    a.pre = pre; a.post = post; a.pre_c0_is_one = pre_c0_is_one(pre);
     const Fr* bufs[3] = {d_src, d_tmp, d_dst};
     const size_t strides[3] = {src_stride, tmp_stride, dst_stride};
     for (int idx = 0; idx < p->npass; ++idx) {
@@ -467,11 +440,13 @@ int ntt_run_sharded(NttPlan* const* plans, int ndev, const int* dev_ids, const F
         for (int g = 0; g < ndev; ++g) {
             PassArgs a;
             memset(&a, 0, sizeof a);
-            a.pre = pre; a.post = post;
+            a.pre = pre; a.post = post; a.pre_c0_is_one = pre_c0_is_one(pre);
             const PassRole r = fill_pass(plans[g], idx, n_in, a);
-            uint32_t threads; size_t smem;
-            if (!plan_pass_v2(a, r.lines, 1, &threads, &smem) || threads > 256 || smem > 200 * 1024) { cudaSetDevice(cur); set_error("sharded ntt: pass %d of 2^%u is too small to shard", idx, log_n); return -1; }
-            const uint64_t blocks = r.lines >> a.log_g;
+            const NttPassGeom geo = ntt_pass_geometry(a.logm, a.inner_cnt, r.lines, 1, sm_count());
+            const uint32_t threads = geo.threads; const size_t smem = geo.smem;
+            if (geo.kernel != 2 || threads > 256 || smem > 200 * 1024) { cudaSetDevice(cur); set_error("sharded ntt: pass %d of 2^%u is too small to shard", idx, log_n); return -1; }
+            a.log_g = geo.log_g;
+            const uint64_t blocks = geo.grid_x;
             if (blocks % (uint64_t)ndev) { cudaSetDevice(cur); set_error("sharded ntt: %llu CTAs do not divide over %d devices", (unsigned long long)blocks, ndev); return -1; }
             a.peer_on = 1; a.log_slice = log_n - log_d; a.block0 = (uint32_t)(blocks / ndev * g);
             for (int h = 0; h < ndev; ++h) { a.src_peers[h] = bufs_r[r.in_buf][h]; a.dst_peers[h] = const_cast<Fr*>(bufs_r[r.out_buf][h]); }

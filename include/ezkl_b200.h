@@ -132,7 +132,8 @@ int b200_coeff_to_extended_batch(const b200_fr* const* coeffs, size_t batch, siz
 /* extended_to_coeff: ifft over the extended domain, * divisor, undo the zeta coset; caller truncates */
 int b200_extended_to_coeff(b200_fr* a, uint32_t ext_k, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, const b200_fr* zeta);
 /* device-resident generic transform: dst[p][j] = post(j) * sum_{i<n_in} pre(i) src[p][i] omega^(ij).
- * pre/post: mode 0 none, 1 constant c[0], 3 cycle c[i mod 3]; c points to HOST constants. tmp: 2^log_n * batch scratch. */
+ * pre/post: mode 0 none, 1 constant c[0], 3 cycle c[i mod 3]; c points to HOST constants. tmp: 2^log_n * batch scratch.
+ * batch <= 65535; with batch > 1, src_stride >= n_in and dst_stride >= 2^log_n (polynomials do not overlap). */
 int b200_ntt_dev(const void* d_src, size_t src_stride, size_t n_in, void* d_tmp, void* d_dst, size_t dst_stride, uint32_t log_n,
                  const b200_fr* omega, int pre_mode, const b200_fr* pre, int post_mode, const b200_fr* post, size_t batch, void* stream);
 
