@@ -94,7 +94,7 @@ struct Ctx {
     bool has_last = false;
     void release() {
         cudaSetDevice(dev);
-        DevBuf* bufs[] = {&msm_ws.counts, &msm_ws.offs, &msm_ws.ents, &msm_ws.subs, &msm_ws.sums, &msm_ws.misc, &poly_ws.scratch, &quot_ws.prog,
+        DevBuf* bufs[] = {&msm_ws.counts, &msm_ws.offs, &msm_ws.ents, &msm_ws.subs, &msm_ws.sums, &msm_ws.misc, &msm_ws.tile_counts, &poly_ws.scratch, &quot_ws.prog,
                           &stage_a, &stage_b, &stage_c, &small};
         for (DevBuf* b : bufs) b->release();
         ring.release(); poly_ws.ring.release(); quot_ws.ring.release();

@@ -26,6 +26,21 @@ __global__ void k_dbg_g1(int op, const G1Affine* a, const G1Affine* b, G1Affine*
     else r = g1_add_mixed(g1_to_xyzz(p), g1_neg(p));
     o[i] = g1_to_affine(r);
 }
+__global__ void k_dbg_xyzz_to_affine(const G1Xyzz* p, G1Affine* o, size_t n) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) o[i] = g1_to_affine(p[i]);
+}
+// What msm.cu (linked into this library for b200_debug_msm_base_off) needs from the product's capi.cu: default tuning, the SM count,
+// and no event profiling.
+static Config g_dbg_cfg;
+const Config& config() { return g_dbg_cfg; }
+int sm_count() {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) return 132;
+    return v;
+}
+bool prof_enabled() { return false; }
+void prof_mark(int, cudaStream_t, bool) {}
 __global__ void k_dbg_digits(const Fr* s, int c, int W, int32_t* out, size_t n) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -218,6 +233,44 @@ int b200_debug_digit_slots_host(const b200_fr* s_canonical, size_t n, int c, int
 int b200_debug_msm_pick_levels(size_t n, int c, size_t max_table_bytes, int* s, int* L) {
     msm_pick_levels(n, c, max_table_bytes, s, L);
     return 0;
+}
+// host-only: the recoding tile policy (msm.cuh): out = {tile, tiles}; tile = 0 when the global-atomic recoding runs
+int b200_debug_msm_recode_plan(size_t n, int batch, uint32_t nbuckets, int W, int sm_count, uint32_t* out /* 2 */) {
+    const MsmRecodePlan p = msm_pick_recode(n, batch, nbuckets, W, sm_count);
+    out[0] = p.tile; out[1] = p.tiles;
+    return 0;
+}
+// msm_run with base_off > 0 (the base-split MSM that only a multi-device call makes in the product) on the current device.
+// scalars [batch][n] and bases [table_n] are HOST arrays; out[b] = sum_i scalars[b][i] * bases[base_off + i] in affine form.
+// The table is built with window c under max_table_bytes (0: every level).  The MSM code is msm.cu, linked into this library.
+int b200_debug_msm_base_off(const b200_fr* scalars, size_t n, int batch, const b200_g1_affine* bases, size_t table_n, int c,
+                            size_t max_table_bytes, size_t base_off, b200_g1_affine* out) {
+    if (n == 0 || batch < 1 || batch > 4096 || base_off + n > table_n || c < 4 || c > 22) return -1;
+    MsmTable t;
+    MsmWorkspace ws;
+    void *d_sc = nullptr, *d_xyzz = nullptr, *d_aff = nullptr;
+    auto run = [&]() -> int {
+        if (int rc = msm_table_alloc(&t, table_n, c, max_table_bytes ? max_table_bytes : ~(size_t)0)) return rc;
+        B200_CUDA(cudaMemcpy(t.d_table, bases, sizeof(G1Affine) * table_n, cudaMemcpyHostToDevice));
+        if (int rc = msm_table_build(&t, nullptr, 0)) return rc;
+        B200_CUDA(cudaMalloc(&d_sc, sizeof(Fr) * n * batch));
+        B200_CUDA(cudaMalloc(&d_xyzz, sizeof(G1Xyzz) * batch));
+        B200_CUDA(cudaMalloc(&d_aff, sizeof(G1Affine) * batch));
+        B200_CUDA(cudaMemcpy(d_sc, scalars, sizeof(Fr) * n * batch, cudaMemcpyHostToDevice));
+        if (int rc = msm_run(t, (const Fr*)d_sc, n, n, batch, (G1Xyzz*)d_xyzz, ws, 0, base_off)) return rc;
+        k_dbg_xyzz_to_affine<<<div_up(batch, 32), 32>>>((const G1Xyzz*)d_xyzz, (G1Affine*)d_aff, (size_t)batch);
+        B200_CUDA(cudaGetLastError());
+        B200_CUDA(cudaMemcpy(out, d_aff, sizeof(G1Affine) * batch, cudaMemcpyDeviceToHost));
+        return 0;
+    };
+    const int rc = run();
+    DevBuf* bufs[] = {&ws.counts, &ws.offs, &ws.ents, &ws.subs, &ws.sums, &ws.misc, &ws.tile_counts};
+    for (DevBuf* b : bufs) b->release();
+    msm_table_free(&t);
+    if (d_sc) cudaFree(d_sc);
+    if (d_xyzz) cudaFree(d_xyzz);
+    if (d_aff) cudaFree(d_aff);
+    return rc;
 }
 // host-only: the NTT pass geometry (ntt.cuh) of a 2^log_n transform of `batch` polynomials on a device of `sm_count` SMs.
 // out[pass * 7 + {0..6}] = kernel (1: k_ntt_pass, 2: k_ntt_pass2), logm, log_g, threads, dynamic shared memory bytes, grid.x,

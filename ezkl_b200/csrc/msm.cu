@@ -6,8 +6,9 @@
 //
 // Pipeline for a batch of `batch` scalar columns sharing one base table (grid.y = column):
 //   1 k_digits<false>   scalar -> canonical -> W signed c-bit digits; per-bucket histogram (warp-aggregated REDs)
+//                       (<= 2^15 buckets: k_digits_tile<false> with shared counters per tile of scalars + k_tile_prefix)
 //   2 k_scan_buckets    exclusive scan of bucket sizes; splits every bucket into chunks of <= cap entries
-//   3 k_digits<true>    same recoding, scatters (table index | sign) into bucket-sorted order
+//   3 k_digits<true>    same recoding, scatters (table index | sign) into bucket-sorted order  (or k_digits_tile<true>)
 //   4 k_fill_chunks     chunk table + histogram of chunk lengths;  5 k_len_offsets;  6 k_order_chunks
 //                       (counting sort of chunks by length, longest first => every warp runs equal-length loops)
 //   7 k_accumulate      one thread per chunk: XYZZ += affine table entry (8M+2S), next base prefetched
@@ -81,7 +82,7 @@ void msm_table_free(MsmTable* t) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// 1 / 3: digit extraction, histogram and scatter.  SUBWIN (s > 1 windows per table level): window w reads level j = w / s and
+// 1 / 3: digit extraction, histogram and scatter with global atomics, for bucket sets too large for k_digits_tile.  SUBWIN (s > 1 windows per table level): window w reads level j = w / s and
 // counts into bucket set r = w % s, i.e. bucket r * 2^(c-1) + |d| - 1; without it j = w, r = 0 (the full table).
 template <bool SCATTER, bool SUBWIN>
 __global__ void __launch_bounds__(256) k_digits(const Fr* __restrict__ scalars, size_t stride, uint32_t n, uint32_t table_n, uint32_t base_off, int c, int W,
@@ -126,6 +127,69 @@ __global__ void __launch_bounds__(256) k_digits(const Fr* __restrict__ scalars, 
             if (SUBWIN) slot.next(c, wpl);
         }
     }
+}
+
+// 1 / 3 with the counters in shared memory (msm_pick_recode: nb <= MSM_TILE_MAX_BUCKETS).  CTA (x, col) recodes its tile of `tile`
+// scalars with one shared counter per bucket.  Counting pass: count, then write the tile's counts to tile_counts[col][x][.].
+// Placement pass: start each counter at offs[b] + (entries of bucket b in the column's earlier tiles), which k_tile_prefix left in
+// tile_counts, and place every entry at its counter's old value.  No global atomics; the entry encoding is k_digits'.
+template <bool SCATTER, bool SUBWIN>
+__global__ void __launch_bounds__(MSM_TILE_THREADS, 1) k_digits_tile(const Fr* __restrict__ scalars, size_t stride, uint32_t n, uint32_t table_n, uint32_t base_off,
+                                                                     int c, int W, uint32_t nbuckets, uint32_t tile, uint32_t* __restrict__ tile_counts /*[col][tiles][nbuckets]*/,
+                                                                     const uint32_t* __restrict__ offs /*[col][nbuckets+1]*/, uint32_t* __restrict__ ents, size_t ent_stride, int wpl) {
+    extern __shared__ uint32_t sh_cnt[];    // nbuckets
+    const uint32_t col = blockIdx.y;
+    const Fr* sc = scalars + (size_t)col * stride;
+    uint32_t* tc = tile_counts + ((size_t)col * gridDim.x + blockIdx.x) * nbuckets;
+    if (SCATTER) {
+        const uint32_t* off = offs + (size_t)col * (nbuckets + 1);
+        for (uint32_t b = threadIdx.x; b < nbuckets; b += blockDim.x) sh_cnt[b] = off[b] + tc[b];
+    } else {
+        for (uint32_t b = threadIdx.x; b < nbuckets; b += blockDim.x) sh_cnt[b] = 0;
+    }
+    __syncthreads();
+    uint32_t* ent = SCATTER ? ents + (size_t)col * ent_stride : nullptr;
+    const uint32_t lo = blockIdx.x * tile, hi = min(lo + tile, n);
+    for (uint32_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+        Fr s = fp_from_mont(fp_load(sc + i));
+        uint32_t carry = 0;
+        MsmWindowSlot slot;
+#pragma unroll 1
+        for (int w = 0; w < W; ++w) {
+            const int32_t d = msm_next_digit(s.l, c, &carry);
+            if (d != 0) {
+                const uint32_t bucket = (SUBWIN ? slot.set_off : 0u) + (uint32_t)(d < 0 ? -d : d) - 1u;
+                const uint32_t pos = atomicAdd(&sh_cnt[bucket], 1u);
+                if (SCATTER) ent[pos] = ((SUBWIN ? slot.level : (uint32_t)w) * table_n + base_off + i) | (d < 0 ? 0x80000000u : 0u);
+            }
+            if (SUBWIN) slot.next(c, wpl);
+        }
+    }
+    if (!SCATTER) {
+        __syncthreads();
+        for (uint32_t b = threadIdx.x; b < nbuckets; b += blockDim.x) tc[b] = sh_cnt[b];
+    }
+}
+
+// 1b (shared-counter path): per bucket, the exclusive prefix of the tile counts over the column's tiles, in place, and the column's
+// total into hist[col][b], which is what k_scan_buckets reads.  Consecutive threads take consecutive buckets (coalesced rows).
+__global__ void __launch_bounds__(256) k_tile_prefix(uint32_t* __restrict__ tile_counts, uint32_t tiles, uint32_t nbuckets, uint32_t* __restrict__ hist) {
+    const uint32_t col = blockIdx.y;
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nbuckets) return;
+    uint32_t* tc = tile_counts + (size_t)col * tiles * nbuckets + b;
+    uint32_t acc = 0;
+    for (uint32_t t0 = 0; t0 < tiles; t0 += 8) {
+        uint32_t v[8];              // eight loads in flight before the stores, which the compiler may not move them past
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = t0 + j < tiles ? tc[(size_t)(t0 + j) * nbuckets] : 0u;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            if (t0 + j < tiles) tc[(size_t)(t0 + j) * nbuckets] = acc;
+            acc += v[j];
+        }
+    }
+    hist[(size_t)col * nbuckets + b] = acc;
 }
 
 // 2: one block per column. offs = exclusive scan of counts; chunk_offs = exclusive scan of ceil(count / cap).
@@ -479,7 +543,8 @@ static uint32_t pick_cap(size_t total_entries) {
 size_t msm_workspace_per_column(const MsmTable& t, size_t n) {
     const size_t nb = (size_t)t.s << (t.c - 1), ents = n * t.W;      // s bucket sets per column
     const size_t chunk_stride = nb + ents / 16 + 1;
-    return ents * 4 + chunk_stride * (12 + sizeof(G1Xyzz)) + nb * (sizeof(G1Xyzz) + 24) + 65536 * (size_t)t.s;
+    const size_t tile_counts = nb <= MSM_TILE_MAX_BUCKETS ? (ents + nb) * 4 : 0;     // msm_pick_recode bounds tiles * nb by ents + nb
+    return ents * 4 + chunk_stride * (12 + sizeof(G1Xyzz)) + nb * (sizeof(G1Xyzz) + 24) + 65536 * (size_t)t.s + tile_counts;
 }
 
 int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int batch, G1Xyzz* d_out, MsmWorkspace& ws, cudaStream_t st, size_t base_off) {
@@ -519,7 +584,10 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     uint32_t final_threads = 32;
     while (final_threads < (uint32_t)TREE_THREADS && final_threads < nparts) final_threads <<= 1;
 
-    // counts region (zeroed every call): hist | cursor | len_hist | len_cursor | heavy
+    const unsigned sms = (unsigned)sm_count();
+    const MsmRecodePlan rp = msm_pick_recode(n, batch, nb, W, (int)sms);
+    // counts region: hist | cursor | len_hist | len_cursor | heavy, zeroed every call (hist first: k_scan_buckets reads it as uint4).
+    // The shared-counter path writes every hist word (k_tile_prefix) and has no cursor, so it zeroes from len_hist on.
     const size_t n_hist = (size_t)batch * nb, n_len = (size_t)batch * (cap + 1), n_heavy = (size_t)batch * heavy_stride;
     const size_t counts_words = 2 * n_hist + 2 * n_len + n_heavy;
     if (ws.counts.ensure(counts_words * 4)) return -2;
@@ -528,6 +596,21 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     uint32_t* len_hist = cursor + n_hist;
     uint32_t* len_cursor = len_hist + n_len;
     uint32_t* heavy = len_cursor + n_len;
+    uint32_t* zero_from = rp.tile ? len_hist : hist;
+    const size_t zero_words = counts_words - (size_t)(zero_from - hist);
+    uint32_t* tile_counts = nullptr;
+    const size_t tile_smem = (size_t)nb * 4;
+    auto* count_k = s == 1 ? k_digits_tile<false, false> : k_digits_tile<false, true>;
+    auto* place_k = s == 1 ? k_digits_tile<true, false> : k_digits_tile<true, true>;
+    if (rp.tile) {
+        if (ws.tile_counts.ensure((size_t)batch * rp.tiles * nb * 4)) return -2;
+        tile_counts = ws.tile_counts.as<uint32_t>();
+        // the attribute belongs to the function on this device, not to the call: always the same limit, so concurrent callers with
+        // other bucket counts cannot lower it under each other's launches (each launch still reserves only nb * 4 bytes)
+        const int smem_limit = (int)(MSM_TILE_MAX_BUCKETS * 4);
+        B200_CUDA(cudaFuncSetAttribute(count_k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit));
+        B200_CUDA(cudaFuncSetAttribute(place_k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit));
+    }
     // offsets: offs | chunk_offs | len_offs
     const size_t n_off = (size_t)batch * (nb + 1);
     if (ws.offs.ensure((2 * n_off + n_len + (size_t)batch) * 4)) return -2;
@@ -550,20 +633,30 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     G1Xyzz* reduced = s > 1 ? partials + (size_t)vcols * nparts : d_out;
 
     ProfScope ps_total(PROF_MSM_TOTAL, st);
-    B200_CUDA(cudaMemsetAsync(hist, 0, counts_words * 4, st));
+    B200_CUDA(cudaMemsetAsync(zero_from, 0, zero_words * 4, st));
     if (prof_enabled()) prof_mark(PROF_MSM_RECODE, st, true);
-    const unsigned sms = (unsigned)sm_count();
     const unsigned dig_blocks = min(div_up(n, 256), sms * 8u);
-    dim3 gd(dig_blocks, batch);
-    if (s == 1) k_digits<false, false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr, 1);
-    else k_digits<false, true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr, s);
-    count_launch();
+    const dim3 gd(dig_blocks, batch), gt(rp.tiles, batch);
+    if (rp.tile) {
+        count_k<<<gt, MSM_TILE_THREADS, tile_smem, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, rp.tile, tile_counts, nullptr, nullptr, 0, s);
+        count_launch();
+        k_tile_prefix<<<dim3(div_up(nb, 256), batch), 256, 0, st>>>(tile_counts, rp.tiles, nb, hist); count_launch();
+    } else {
+        if (s == 1) k_digits<false, false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr, 1);
+        else k_digits<false, true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, hist, nullptr, nullptr, 0, nullptr, s);
+        count_launch();
+    }
     {
         ProfScope ps(PROF_MSM_SCAN, st);
         k_scan_buckets<<<batch, 1024, 0, st>>>(hist, offs, chunk_offs, nb, cap, skew); count_launch();
     }
-    if (s == 1) k_digits<true, false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew, 1);
-    else k_digits<true, true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew, s);
+    if (rp.tile) {
+        place_k<<<gt, MSM_TILE_THREADS, tile_smem, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, rp.tile, tile_counts, offs, ents, ent_stride, s);
+    } else if (s == 1) {
+        k_digits<true, false><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew, 1);
+    } else {
+        k_digits<true, true><<<gd, 256, 0, st>>>(d_scalars, stride, (uint32_t)n, (uint32_t)t.n, (uint32_t)base_off, c, W, nb, cursor, offs, ents, ent_stride, skew, s);
+    }
     count_launch();
     k_fill_chunks<<<dim3(div_up(nb, 256), batch), 256, (cap + 1) * 4, st>>>(offs, chunk_offs, nb, cap, chunk_start, chunk_len, chunk_stride, len_hist, heavy, heavy_stride); count_launch();
     k_len_offsets<<<batch, 32, 0, st>>>(len_hist, len_offs, cap); count_launch();

@@ -22,7 +22,7 @@ struct MsmTable {
 };
 
 struct MsmWorkspace {
-    DevBuf counts, offs, ents, subs, sums, misc;
+    DevBuf counts, offs, ents, subs, sums, misc, tile_counts;
 };
 
 int msm_default_window(size_t n);
@@ -35,6 +35,38 @@ inline void msm_pick_levels(size_t n, int c, size_t max_table_bytes, int* s, int
         const int l = (W + k - 1) / k;
         if (k == W || (size_t)l * level_bytes <= max_table_bytes) { *s = k; *L = l; return; }
     }
+}
+// Recoding with the bucket counters in shared memory (k_digits_tile): CTA (x, col) recodes the `tile` scalars [x * tile, (x + 1) * tile)
+// of column col, `tiles` = ceil(n / tile) CTAs per column, and holds one 32-bit counter per bucket of the column.  Both recoding
+// passes take this plan, so they cut the columns into the same tiles.  tile = 0: the bucket set does not fit in shared memory and the
+// global-atomic k_digits runs instead.
+struct MsmRecodePlan {
+    uint32_t tile = 0, tiles = 0;
+};
+static constexpr uint32_t MSM_TILE_MAX_BUCKETS = 1u << 15;      // 128 KiB of counters, one CTA per SM
+static constexpr uint32_t MSM_TILE_THREADS = 1024;
+static constexpr size_t MSM_TILE_L2_BYTES = (size_t)16 << 20;   // entry-list bytes the placement pass may scatter into at once (of a 50 MB L2)
+// Pure host function of the call shape and the SM count.  The tile is chosen so that
+//   - the columns in flight (one CTA per SM) scatter into at most MSM_TILE_L2_BYTES of entry list, so the random 4-byte writes
+//     merge in L2: tiles >= sms * n * W * 4 / MSM_TILE_L2_BYTES;
+//   - a small batch still has one CTA per SM: tiles >= sms / batch;
+//   - a tile makes at least as many entries (tile * W) as it has counters to clear and publish: tile >= nb / W.  This also keeps the
+//     [col][tile][bucket] count matrix (tiles * nb words) no larger than n * W + nb words per column (msm_workspace_per_column);
+// with the tile a multiple of the CTA size.
+inline MsmRecodePlan msm_pick_recode(size_t n, int batch, uint32_t nb, int W, int sms) {
+    MsmRecodePlan p;
+    if (n == 0 || batch < 1 || W < 1 || sms < 1 || nb == 0 || nb > MSM_TILE_MAX_BUCKETS) return p;
+    const size_t ents = n * (size_t)W;
+    size_t tiles = ((size_t)sms * ents * 4 + MSM_TILE_L2_BYTES - 1) / MSM_TILE_L2_BYTES;
+    const size_t fill = ((size_t)sms + batch - 1) / batch;
+    if (tiles < fill) tiles = fill;
+    size_t tile = (n + tiles - 1) / tiles;
+    const size_t min_tile = (nb + W - 1) / W;
+    if (tile < min_tile) tile = min_tile;
+    tile = (tile + MSM_TILE_THREADS - 1) / MSM_TILE_THREADS * MSM_TILE_THREADS;
+    p.tile = (uint32_t)tile;
+    p.tiles = (uint32_t)((n + tile - 1) / tile);
+    return p;
 }
 // Picks the window (c <= 0: msm_default_window) and the level count, and allocates the table.  Level 0 (the first n points)
 // is left for the caller to fill, e.g. by uploading the bases straight into it.
