@@ -1151,6 +1151,8 @@ int b200_prefix_scan(int product, const b200_fr* a, size_t n, const b200_fr* ini
 }
 static int kate_division_on(Ctx* c, cudaStream_t st, const void* d_a, size_t n, const b200_fr* b, void* d_q) {
     B200_CHECK(d_a && b && d_q, -1, "kate_division: null pointer");
+    // q[e] is computed from a[e + 1 ..]: a thread's stores would overwrite the coefficient its neighbour still has to read
+    B200_CHECK(d_q != d_a, -1, "kate_division: q must not alias a (the quotient cannot be computed in place)");
     const Fr bv = as_fr(b);
     return poly_kate_division(reinterpret_cast<const Fr*>(d_a), n, &bv, reinterpret_cast<Fr*>(d_q), c->poly_ws, st);
 }

@@ -164,13 +164,15 @@ int b200_poly_eval_batch_dev(const void* d_polys, size_t stride, size_t n, const
 /* ff::BatchInvert (zeros stay zero) */
 int b200_batch_invert(b200_fr* a, size_t n);
 int b200_batch_invert_dev(void* d_a, size_t n, void* stream);
-/* out[0] = init, out[i+1] = out[i] (* or +) a[i]: permutation z(X) / mv-lookup phi(X) running columns */
+/* out[0] = init, out[i+1] = out[i] (* or +) a[i]: permutation z(X) / mv-lookup phi(X) running columns.  The _dev forms may run in
+ * place (d_out == d_a, and for the batch form out_stride == a_stride): every element is read by the thread that overwrites it. */
 int b200_prefix_scan(int product, const b200_fr* a, size_t n, const b200_fr* init, b200_fr* out);
 int b200_prefix_scan_dev(int product, const void* d_a, size_t n, const b200_fr* init, void* d_out, void* stream);
 /* `batch` independent columns in one call (the mv-lookup grand sums of a proof are independent of each other; the permutation products are
  * chained through last_z and are not): column p at d_a + p * a_stride elements, its result at d_out + p * out_stride, initial value inits[p] */
 int b200_prefix_scan_batch_dev(int product, const void* d_a, size_t a_stride, size_t n, size_t batch, const b200_fr* inits, void* d_out, size_t out_stride, void* stream);
-/* kate_division(a, b): quotient of a(X) by (X - b), n-1 coefficients */
+/* kate_division(a, b): quotient of a(X) by (X - b), n-1 coefficients.  Not in place: q[e] depends on a[e+1 ..], so the _dev form
+ * returns -1 when d_q == d_a. */
 int b200_kate_division(const b200_fr* a, size_t n, const b200_fr* b, b200_fr* q);
 int b200_kate_division_dev(const void* d_a, size_t n, const b200_fr* b, void* d_q, void* stream);
 
