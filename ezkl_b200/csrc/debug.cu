@@ -1,6 +1,6 @@
 // debug.cu — small self-test entry points (b200_debug_*) used only by tests/ to localise a failure to one layer
 // (field arithmetic, group law, digit recoding) before the composite kernels are blamed.  Not part of the drop-in ABI.
-#include "../../include/ezkl_b200.h"
+#include "debug.h"
 #include "msm.cuh"
 #include "ntt.cuh"
 

@@ -19,8 +19,7 @@ from . import fields as F
 def _stream():
     """torch's current stream as a cudaStream_t.  The legacy default stream has handle 0, which the C ABI reads as "use the
     library's own stream"; pass CUDA's explicit cudaStreamLegacy handle (0x1) instead so ordering and event timing hold."""
-    h = torch.cuda.current_stream().cuda_stream
-    return C.c_void_p(h if h else 1)
+    return torch.cuda.current_stream().cuda_stream or 1
 
 
 def _chk(t: torch.Tensor, last: int):
@@ -34,7 +33,7 @@ def _host_fr(x) -> np.ndarray:
 def generate_bases(n: int, seed: int = 0xE2C1B200) -> torch.Tensor:
     nat.ensure_init()
     out = torch.empty((n, 8), dtype=torch.int64, device="cuda")
-    nat.check(nat.lib().b200_g1_generate_dev(C.c_uint64(seed), C.c_size_t(n), nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_g1_generate_dev(seed, n, out.data_ptr(), _stream()))
     return out
 
 
@@ -46,7 +45,7 @@ def fixed_base_mul(scalars: torch.Tensor, base=None) -> torch.Tensor:
         base = np.concatenate([F.fq_to_limbs(1), F.fq_to_limbs(2)])
     base = nat.as_u64(base, 8)
     out = torch.empty((n, 8), dtype=torch.int64, device="cuda")
-    nat.check(nat.lib().b200_g1_fixed_base_mul_dev(nat.dev(scalars.data_ptr()), C.c_size_t(n), nat.ptr(base), nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_g1_fixed_base_mul_dev(scalars.data_ptr(), n, nat.ptr(base), out.data_ptr(), _stream()))
     return out
 
 
@@ -100,8 +99,7 @@ class DeviceBases:
         self.n = d_points.shape[0]
         torch.cuda.current_stream().synchronize()
         h = C.c_uint64(0)
-        nat.check(nat.lib().b200_bases_register_ex_dev(nat.dev(d_points.data_ptr()), C.c_size_t(self.n), C.c_int(window_bits),
-                                                        C.c_size_t(max_table_bytes), C.byref(h)))
+        nat.check(nat.lib().b200_bases_register_ex_dev(d_points.data_ptr(), self.n, window_bits, max_table_bytes, C.byref(h)))
         self.handle = h.value
 
     def info(self) -> dict:
@@ -110,7 +108,7 @@ class DeviceBases:
 
     def release(self):
         if self.handle:
-            nat.check(nat.lib().b200_bases_release(C.c_uint64(self.handle)))
+            nat.check(nat.lib().b200_bases_release(self.handle))
             self.handle = 0
 
 
@@ -122,8 +120,7 @@ def msm_batch(bases: DeviceBases, scalars: torch.Tensor, out: torch.Tensor | Non
     batch, n = scalars.shape[0], scalars.shape[1]
     if out is None:
         out = torch.empty((batch, 16), dtype=torch.int64, device="cuda")
-    nat.check(nat.lib().b200_msm_batch_dev(C.c_uint64(bases.handle), nat.dev(scalars.data_ptr()), C.c_size_t(n), C.c_size_t(n), C.c_size_t(batch),
-                                           nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_msm_batch_dev(bases.handle, scalars.data_ptr(), n, n, batch, out.data_ptr(), _stream()))
     return out
 
 
@@ -132,7 +129,7 @@ def g1_sum(points: torch.Tensor) -> torch.Tensor:
     _chk(points, 16)
     groups, count = points.shape[0], points.shape[1]
     out = torch.empty((groups, 16), dtype=torch.int64, device="cuda")
-    nat.check(nat.lib().b200_g1_sum_dev(nat.dev(points.data_ptr()), C.c_size_t(groups), C.c_size_t(count), nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_g1_sum_dev(points.data_ptr(), groups, count, out.data_ptr(), _stream()))
     return out
 
 
@@ -140,7 +137,7 @@ def normalize(points_xyzz: torch.Tensor) -> np.ndarray:
     """Device XYZZ [m,16] -> host normalised Jacobian wire [m,12] (synchronises)."""
     h = points_xyzz.cpu().numpy().view(np.uint64).reshape(-1, 16)
     out = np.zeros((h.shape[0], 12), np.uint64)
-    nat.check(nat.lib().b200_g1_normalize(nat.ptr(np.ascontiguousarray(h)), C.c_size_t(h.shape[0]), nat.ptr(out)))
+    nat.check(nat.lib().b200_g1_normalize(nat.ptr(np.ascontiguousarray(h)), h.shape[0], nat.ptr(out)))
     return out
 
 
@@ -159,9 +156,9 @@ def ntt(src: torch.Tensor, log_n: int, omega, *, n_in: int | None = None, pre=No
         tmp = torch.empty((batch, N, 4), dtype=torch.int64, device="cuda")
     pre_a = np.ascontiguousarray(np.stack([_host_fr(c) for c in pre])) if pre is not None else None
     post_a = np.ascontiguousarray(np.stack([_host_fr(c) for c in post])) if post is not None else None
-    nat.check(nat.lib().b200_ntt_dev(nat.dev(src.data_ptr()), C.c_size_t(n_src), C.c_size_t(n_in), nat.dev(tmp.data_ptr()), nat.dev(out.data_ptr()), C.c_size_t(N),
-                                     C.c_uint32(log_n), nat.ptr(_host_fr(omega)), C.c_int(0 if pre is None else len(pre)), nat.ptr(pre_a) if pre is not None else None,
-                                     C.c_int(0 if post is None else len(post)), nat.ptr(post_a) if post is not None else None, C.c_size_t(batch), _stream()))
+    nat.check(nat.lib().b200_ntt_dev(src.data_ptr(), n_src, n_in, tmp.data_ptr(), out.data_ptr(), N,
+                                     log_n, nat.ptr(_host_fr(omega)), 0 if pre is None else len(pre), nat.ptr(pre_a) if pre is not None else None,
+                                     0 if post is None else len(post), nat.ptr(post_a) if post is not None else None, batch, _stream()))
     return out
 
 
@@ -174,8 +171,7 @@ def poly_op(op: str, a: torch.Tensor, b: torch.Tensor | None = None, s=None, out
         out = torch.empty_like(a)
     n = a.numel() // 4
     sp = nat.ptr(_host_fr(s)) if s is not None else None
-    nat.check(nat.lib().b200_poly_op_dev(C.c_int(_OPS[op]), nat.dev(a.data_ptr()), nat.dev(b.data_ptr()) if b is not None else None, sp,
-                                         nat.dev(out.data_ptr()), C.c_size_t(n), _stream()))
+    nat.check(nat.lib().b200_poly_op_dev(_OPS[op], a.data_ptr(), b.data_ptr() if b is not None else None, sp, out.data_ptr(), n, _stream()))
     return out
 
 
@@ -190,14 +186,14 @@ def lincomb(polys, scalars, out: torch.Tensor | None = None) -> torch.Tensor:
     if out is None:
         out = torch.empty_like(plist[0])
     ptrs = (C.c_void_p * len(plist))(*[p_.data_ptr() for p_ in plist])
-    nat.check(nat.lib().b200_poly_lincomb_dev(ptrs, nat.ptr(sc), C.c_size_t(len(plist)), C.c_size_t(n), nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_poly_lincomb_dev(ptrs, nat.ptr(sc), len(plist), n, out.data_ptr(), _stream()))
     return out
 
 
 def scale_cycle(a: torch.Tensor, consts) -> torch.Tensor:
     _chk(a, 4)
     cs = nat.as_u64(consts, 4)
-    nat.check(nat.lib().b200_poly_scale_cycle_dev(nat.dev(a.data_ptr()), C.c_size_t(a.numel() // 4), nat.ptr(cs), C.c_uint32(cs.shape[0]), _stream()))
+    nat.check(nat.lib().b200_poly_scale_cycle_dev(a.data_ptr(), a.numel() // 4, nat.ptr(cs), cs.shape[0], _stream()))
     return a
 
 
@@ -207,13 +203,13 @@ def eval_batch(polys: torch.Tensor, xs) -> torch.Tensor:
     batch, n = polys.shape[0], polys.shape[1]
     xs = nat.as_u64(xs, 4)
     out = torch.empty((batch, 4), dtype=torch.int64, device="cuda")
-    nat.check(nat.lib().b200_poly_eval_batch_dev(nat.dev(polys.data_ptr()), C.c_size_t(n), C.c_size_t(n), nat.ptr(xs), C.c_size_t(batch), nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_poly_eval_batch_dev(polys.data_ptr(), n, n, nat.ptr(xs), batch, out.data_ptr(), _stream()))
     return out
 
 
 def batch_invert(a: torch.Tensor) -> torch.Tensor:
     _chk(a, 4)
-    nat.check(nat.lib().b200_batch_invert_dev(nat.dev(a.data_ptr()), C.c_size_t(a.numel() // 4), _stream()))
+    nat.check(nat.lib().b200_batch_invert_dev(a.data_ptr(), a.numel() // 4, _stream()))
     return a
 
 
@@ -221,8 +217,7 @@ def prefix_scan(a: torch.Tensor, init, product: bool, out: torch.Tensor | None =
     _chk(a, 4)
     if out is None:
         out = torch.empty_like(a)
-    nat.check(nat.lib().b200_prefix_scan_dev(C.c_int(1 if product else 0), nat.dev(a.data_ptr()), C.c_size_t(a.numel() // 4), nat.ptr(_host_fr(init)),
-                                             nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_prefix_scan_dev(1 if product else 0, a.data_ptr(), a.numel() // 4, nat.ptr(_host_fr(init)), out.data_ptr(), _stream()))
     return out
 
 
@@ -234,8 +229,8 @@ def prefix_scan_batch(a: torch.Tensor, inits, product: bool, out: torch.Tensor |
         out = torch.empty_like(a)
     iv = nat.as_u64(inits, 4)
     assert iv.shape[0] == batch
-    nat.check(nat.lib().b200_prefix_scan_batch_dev(C.c_int(1 if product else 0), nat.dev(a.data_ptr()), C.c_size_t(n), C.c_size_t(n), C.c_size_t(batch), nat.ptr(iv),
-                                                   nat.dev(out.data_ptr()), C.c_size_t(n), _stream()))
+    nat.check(nat.lib().b200_prefix_scan_batch_dev(1 if product else 0, a.data_ptr(), n, n, batch, nat.ptr(iv),
+                                                   out.data_ptr(), n, _stream()))
     return out
 
 
@@ -244,7 +239,7 @@ def kate_division(a: torch.Tensor, b, out: torch.Tensor | None = None) -> torch.
     n = a.numel() // 4
     if out is None:
         out = torch.empty((n - 1, 4), dtype=torch.int64, device="cuda")
-    nat.check(nat.lib().b200_kate_division_dev(nat.dev(a.data_ptr()), C.c_size_t(n), nat.ptr(_host_fr(b)), nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_kate_division_dev(a.data_ptr(), n, nat.ptr(_host_fr(b)), out.data_ptr(), _stream()))
     return out
 
 

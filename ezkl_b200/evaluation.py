@@ -282,9 +282,9 @@ def evaluate_h(program: QuotientProgram, columns, k: int, ext_k: int) -> np.ndar
     assert all(c.shape[0] == N for c in cols)
     loads, consts, prog = program.arrays()
     out = np.zeros((N, 4), np.uint64)
-    nat.check(nat.lib().b200_quotient_eval(nat.ptr_array(cols) if cols else None, C.c_size_t(len(cols)), C.c_uint32(k), C.c_uint32(ext_k),
-                                           loads.ctypes.data_as(C.c_void_p), C.c_size_t(loads.shape[0]), nat.ptr(consts) if consts.size else None,
-                                           C.c_size_t(consts.shape[0]), prog.ctypes.data_as(C.c_void_p), C.c_size_t(prog.shape[0]), nat.ptr(out)))
+    nat.check(nat.lib().b200_quotient_eval(nat.ptr_array(cols) if cols else None, len(cols), k, ext_k,
+                                           loads.ctypes.data_as(C.c_void_p), loads.shape[0], nat.ptr(consts) if consts.size else None,
+                                           consts.shape[0], prog.ctypes.data_as(C.c_void_p), prog.shape[0], nat.ptr(out)))
     return out
 
 
@@ -299,10 +299,10 @@ def evaluate_h_from_polys(program: QuotientProgram, polys, domain, finish: bool 
     loads, consts, prog = program.arrays()
     out = np.zeros((N, 4), np.uint64)
     t_ev = nat.ptr(domain.t_evaluations) if finish else None
-    nat.check(nat.lib().b200_evaluate_h(nat.ptr_array(cols) if cols else None, lens, C.c_size_t(len(cols)), C.c_uint32(domain.k), C.c_uint32(domain.extended_k),
-                                        nat.ptr(domain.extended_omega), nat.ptr(domain.g_coset), loads.ctypes.data_as(C.c_void_p), C.c_size_t(loads.shape[0]),
-                                        nat.ptr(consts) if consts.size else None, C.c_size_t(consts.shape[0]), prog.ctypes.data_as(C.c_void_p), C.c_size_t(prog.shape[0]),
-                                        t_ev, C.c_uint32(domain.t_evaluations.shape[0] if finish else 0), nat.ptr(domain.extended_omega_inv) if finish else None,
+    nat.check(nat.lib().b200_evaluate_h(nat.ptr_array(cols) if cols else None, lens, len(cols), domain.k, domain.extended_k,
+                                        nat.ptr(domain.extended_omega), nat.ptr(domain.g_coset), loads.ctypes.data_as(C.c_void_p), loads.shape[0],
+                                        nat.ptr(consts) if consts.size else None, consts.shape[0], prog.ctypes.data_as(C.c_void_p), prog.shape[0],
+                                        t_ev, domain.t_evaluations.shape[0] if finish else 0, nat.ptr(domain.extended_omega_inv) if finish else None,
                                         nat.ptr(domain.extended_ifft_divisor) if finish else None, nat.ptr(out)))
     return out
 
@@ -318,9 +318,9 @@ def evaluate_h_device(program: QuotientProgram, columns, k: int, ext_k: int, out
         out = torch.empty((N, 4), dtype=torch.int64, device="cuda")
     loads, consts, prog = program.arrays()
     ptrs = (C.c_void_p * max(1, len(columns)))(*[c.data_ptr() for c in columns])
-    nat.check(nat.lib().b200_quotient_eval_dev(ptrs, C.c_size_t(len(columns)), C.c_uint32(k), C.c_uint32(ext_k), loads.ctypes.data_as(C.c_void_p),
-                                               C.c_size_t(loads.shape[0]), nat.ptr(consts) if consts.size else None, C.c_size_t(consts.shape[0]),
-                                               prog.ctypes.data_as(C.c_void_p), C.c_size_t(prog.shape[0]), nat.dev(out.data_ptr()), _stream()))
+    nat.check(nat.lib().b200_quotient_eval_dev(ptrs, len(columns), k, ext_k, loads.ctypes.data_as(C.c_void_p),
+                                               loads.shape[0], nat.ptr(consts) if consts.size else None, consts.shape[0],
+                                               prog.ctypes.data_as(C.c_void_p), prog.shape[0], out.data_ptr(), _stream()))
     return out
 
 
@@ -392,7 +392,7 @@ def lookup_multiplicities(table, inputs, n_rows: int):
     ins = [nat.as_u64(c, 4) for c in inputs]
     m = np.zeros_like(t)
     missing = C.c_uint64(0)
-    nat.check(nat.lib().b200_lookup_multiplicities(nat.ptr(t), C.c_size_t(t.shape[0]), nat.ptr_array(ins), C.c_size_t(len(ins)), C.c_size_t(n_rows), nat.ptr(m), C.byref(missing)))
+    nat.check(nat.lib().b200_lookup_multiplicities(nat.ptr(t), t.shape[0], nat.ptr_array(ins), len(ins), n_rows, nat.ptr(m), C.byref(missing)))
     if missing.value:
         raise nat.B200Error("lookup_multiplicities: %d input cells are not in the table" % missing.value)
     return m

@@ -36,7 +36,7 @@ class Bases:
         pts = nat.as_u64(points, 8)
         self.n = pts.shape[0]
         h = C.c_uint64(0)
-        nat.check(nat.lib().b200_bases_register_ex(nat.ptr(pts), C.c_size_t(self.n), C.c_int(window_bits), C.c_size_t(max_table_bytes), C.byref(h)))
+        nat.check(nat.lib().b200_bases_register_ex(nat.ptr(pts), self.n, window_bits, max_table_bytes, C.byref(h)))
         self.handle = h.value
 
     @classmethod
@@ -45,7 +45,7 @@ class Bases:
         self = cls.__new__(cls)
         self.n = n
         h = C.c_uint64(0)
-        nat.check(nat.lib().b200_bases_register_ex_dev(nat.dev(d_ptr), C.c_size_t(n), C.c_int(window_bits), C.c_size_t(max_table_bytes), C.byref(h)))
+        nat.check(nat.lib().b200_bases_register_ex_dev(d_ptr, n, window_bits, max_table_bytes, C.byref(h)))
         self.handle = h.value
         return self
 
@@ -54,7 +54,7 @@ class Bases:
 
     def release(self):
         if self.handle:
-            nat.check(nat.lib().b200_bases_release(C.c_uint64(self.handle)))
+            nat.check(nat.lib().b200_bases_release(self.handle))
             self.handle = 0
 
 
@@ -62,9 +62,9 @@ def bases_info(handle: int) -> dict:
     """A registered base table: n, window_bits, windows (W), levels (L stored levels), windows_per_level (s) and table_bytes
     (per device)."""
     n, c, w = C.c_size_t(0), C.c_int(0), C.c_int(0)
-    nat.check(nat.lib().b200_bases_info(C.c_uint64(handle), C.byref(n), C.byref(c), C.byref(w)))
+    nat.check(nat.lib().b200_bases_info(handle, C.byref(n), C.byref(c), C.byref(w)))
     lv, wpl, nbytes = C.c_int(0), C.c_int(0), C.c_size_t(0)
-    nat.check(nat.lib().b200_bases_table(C.c_uint64(handle), C.byref(lv), C.byref(wpl), C.byref(nbytes)))
+    nat.check(nat.lib().b200_bases_table(handle, C.byref(lv), C.byref(wpl), C.byref(nbytes)))
     return {"n": n.value, "window_bits": c.value, "windows": w.value, "levels": lv.value, "windows_per_level": wpl.value,
             "table_bytes": nbytes.value}
 
@@ -78,7 +78,7 @@ def best_multiexp(coeffs, bases: Bases) -> np.ndarray:
     if sc.shape[0] > bases.n:
         raise nat.B200Error("best_multiexp: %d coefficients but %d bases" % (sc.shape[0], bases.n))
     out = np.zeros(12, np.uint64)
-    nat.check(nat.lib().b200_msm(C.c_uint64(bases.handle), nat.ptr(sc), C.c_size_t(sc.shape[0]), nat.ptr(out)))
+    nat.check(nat.lib().b200_msm(bases.handle, nat.ptr(sc), sc.shape[0], nat.ptr(out)))
     return out
 
 
@@ -90,7 +90,7 @@ def best_multiexp_batch(columns, bases: Bases) -> np.ndarray:
     n = cols[0].shape[0]
     assert all(c.shape[0] == n for c in cols)
     out = np.zeros((len(cols), 12), np.uint64)
-    nat.check(nat.lib().b200_msm_batch(C.c_uint64(bases.handle), nat.ptr_array(cols), C.c_size_t(n), C.c_size_t(len(cols)), nat.ptr(out)))
+    nat.check(nat.lib().b200_msm_batch(bases.handle, nat.ptr_array(cols), n, len(cols), nat.ptr(out)))
     return out
 
 
@@ -100,7 +100,7 @@ def best_fft(a, omega, log_n: int) -> np.ndarray:
     if a.shape[0] != 1 << log_n:
         raise nat.B200Error("best_fft: len %d != 2^%d" % (a.shape[0], log_n))
     nat.ensure_init()
-    nat.check(nat.lib().b200_fft(nat.ptr(a), C.c_uint32(log_n), nat.ptr(_fr(omega))))
+    nat.check(nat.lib().b200_fft(nat.ptr(a), log_n, nat.ptr(_fr(omega))))
     return a
 
 
@@ -108,7 +108,7 @@ def eval_polynomial(poly, point) -> np.ndarray:
     poly = _fr(poly)
     out = np.zeros(4, np.uint64)
     nat.ensure_init()
-    nat.check(nat.lib().b200_poly_eval(nat.ptr(poly), C.c_size_t(poly.shape[0]), nat.ptr(_fr(point)), nat.ptr(out)))
+    nat.check(nat.lib().b200_poly_eval(nat.ptr(poly), poly.shape[0], nat.ptr(_fr(point)), nat.ptr(out)))
     return out
 
 
@@ -120,7 +120,7 @@ def eval_polynomial_batch(polys, points) -> np.ndarray:
     if not ps:
         return out
     nat.ensure_init()
-    nat.check(nat.lib().b200_poly_eval_batch(nat.ptr_array(ps), C.c_size_t(ps[0].shape[0]), nat.ptr(xs), C.c_size_t(len(ps)), nat.ptr(out)))
+    nat.check(nat.lib().b200_poly_eval_batch(nat.ptr_array(ps), ps[0].shape[0], nat.ptr(xs), len(ps), nat.ptr(out)))
     return out
 
 
@@ -130,14 +130,14 @@ def kate_division(a, b) -> np.ndarray:
         raise nat.B200Error("kate_division: empty polynomial")
     q = np.zeros((a.shape[0] - 1, 4), np.uint64)
     nat.ensure_init()
-    nat.check(nat.lib().b200_kate_division(nat.ptr(a), C.c_size_t(a.shape[0]), nat.ptr(_fr(b)), nat.ptr(q)))
+    nat.check(nat.lib().b200_kate_division(nat.ptr(a), a.shape[0], nat.ptr(_fr(b)), nat.ptr(q)))
     return q
 
 
 def batch_invert(a) -> np.ndarray:
     a = _fr(a).copy()
     nat.ensure_init()
-    nat.check(nat.lib().b200_batch_invert(nat.ptr(a), C.c_size_t(a.shape[0])))
+    nat.check(nat.lib().b200_batch_invert(nat.ptr(a), a.shape[0]))
     return a
 
 
@@ -145,7 +145,7 @@ def prefix_scan(a, init, product: bool) -> np.ndarray:
     a = _fr(a)
     out = np.empty_like(a)
     nat.ensure_init()
-    nat.check(nat.lib().b200_prefix_scan(C.c_int(1 if product else 0), nat.ptr(a), C.c_size_t(a.shape[0]), nat.ptr(_fr(init)), nat.ptr(out)))
+    nat.check(nat.lib().b200_prefix_scan(1 if product else 0, nat.ptr(a), a.shape[0], nat.ptr(_fr(init)), nat.ptr(out)))
     return out
 
 
@@ -159,7 +159,7 @@ def poly_op(op: str, a, b=None, s=None) -> np.ndarray:
     nat.ensure_init()
     bp = nat.ptr(_fr(b)) if b is not None else None
     sp = nat.ptr(_fr(s)) if s is not None else None
-    nat.check(nat.lib().b200_poly_op(C.c_int(_OPS[op]), nat.ptr(a), bp, sp, nat.ptr(out), C.c_size_t(a.shape[0])))
+    nat.check(nat.lib().b200_poly_op(_OPS[op], nat.ptr(a), bp, sp, nat.ptr(out), a.shape[0]))
     return out
 
 
@@ -170,7 +170,7 @@ def poly_lincomb(polys, scalars) -> np.ndarray:
     assert sc.shape[0] == len(ps) and len(ps) > 0
     out = np.zeros_like(ps[0])
     nat.ensure_init()
-    nat.check(nat.lib().b200_poly_lincomb(nat.ptr_array(ps), nat.ptr(sc), C.c_size_t(len(ps)), C.c_size_t(ps[0].shape[0]), nat.ptr(out)))
+    nat.check(nat.lib().b200_poly_lincomb(nat.ptr_array(ps), nat.ptr(sc), len(ps), ps[0].shape[0], nat.ptr(out)))
     return out
 
 
@@ -212,13 +212,13 @@ class EvaluationDomain:
     def lagrange_to_coeff(self, a) -> np.ndarray:
         a = _fr(a).copy()
         assert a.shape[0] == self.n
-        nat.check(nat.lib().b200_ifft(nat.ptr(a), C.c_uint32(self.k), nat.ptr(self.omega_inv), nat.ptr(self.ifft_divisor)))
+        nat.check(nat.lib().b200_ifft(nat.ptr(a), self.k, nat.ptr(self.omega_inv), nat.ptr(self.ifft_divisor)))
         return a
 
     def lagrange_to_coeff_batch(self, cols):
         cols = [_fr(c).copy() for c in cols]
         if cols:
-            nat.check(nat.lib().b200_ifft_batch(nat.ptr_array(cols), C.c_size_t(len(cols)), C.c_uint32(self.k), nat.ptr(self.omega_inv), nat.ptr(self.ifft_divisor)))
+            nat.check(nat.lib().b200_ifft_batch(nat.ptr_array(cols), len(cols), self.k, nat.ptr(self.omega_inv), nat.ptr(self.ifft_divisor)))
         return cols
 
     def coeff_to_lagrange(self, a) -> np.ndarray:
@@ -228,7 +228,7 @@ class EvaluationDomain:
         a = _fr(a)
         assert a.shape[0] == self.n
         out = np.zeros((self.extended_len(), 4), np.uint64)
-        nat.check(nat.lib().b200_coeff_to_extended(nat.ptr(a), C.c_size_t(a.shape[0]), C.c_uint32(self.extended_k), nat.ptr(self.extended_omega),
+        nat.check(nat.lib().b200_coeff_to_extended(nat.ptr(a), a.shape[0], self.extended_k, nat.ptr(self.extended_omega),
                                                     nat.ptr(self.g_coset), nat.ptr(out)))
         return out
 
@@ -236,7 +236,7 @@ class EvaluationDomain:
         cols = [_fr(c) for c in cols]
         outs = [np.zeros((self.extended_len(), 4), np.uint64) for _ in cols]
         if cols:
-            nat.check(nat.lib().b200_coeff_to_extended_batch(nat.ptr_array(cols), C.c_size_t(len(cols)), C.c_size_t(self.n), C.c_uint32(self.extended_k),
+            nat.check(nat.lib().b200_coeff_to_extended_batch(nat.ptr_array(cols), len(cols), self.n, self.extended_k,
                                                               nat.ptr(self.extended_omega), nat.ptr(self.g_coset), nat.ptr_array(outs)))
         return outs
 
@@ -244,14 +244,14 @@ class EvaluationDomain:
         """Returns n * quotient_poly_degree coefficients (upstream truncates the same way)."""
         a = _fr(a).copy()
         assert a.shape[0] == self.extended_len()
-        nat.check(nat.lib().b200_extended_to_coeff(nat.ptr(a), C.c_uint32(self.extended_k), nat.ptr(self.extended_omega_inv),
+        nat.check(nat.lib().b200_extended_to_coeff(nat.ptr(a), self.extended_k, nat.ptr(self.extended_omega_inv),
                                                     nat.ptr(self.extended_ifft_divisor), nat.ptr(self.g_coset)))
         return a[: self.n * self.quotient_poly_degree]
 
     def divide_by_vanishing_poly(self, a) -> np.ndarray:
         a = _fr(a).copy()
         assert a.shape[0] == self.extended_len()
-        nat.check(nat.lib().b200_poly_scale_cycle(nat.ptr(a), C.c_size_t(a.shape[0]), nat.ptr(self.t_evaluations), C.c_uint32(self.t_evaluations.shape[0])))
+        nat.check(nat.lib().b200_poly_scale_cycle(nat.ptr(a), a.shape[0], nat.ptr(self.t_evaluations), self.t_evaluations.shape[0]))
         return a
 
     def keygen_l_polys(self, blinding_factors: int):
@@ -285,7 +285,7 @@ def g_to_lagrange(g, k: int) -> np.ndarray:
     omega = pow(F.FR_ROOT_OF_UNITY, 1 << (F.FR_S - k), r)
     out = np.zeros_like(g)
     nat.ensure_init()
-    nat.check(nat.lib().b200_g1_fft(nat.ptr(g), C.c_uint32(k), nat.ptr(F.fr_to_limbs(F.fr_inv(omega))), nat.ptr(F.fr_to_limbs(F.fr_inv(n))), nat.ptr(out)))
+    nat.check(nat.lib().b200_g1_fft(nat.ptr(g), k, nat.ptr(F.fr_to_limbs(F.fr_inv(omega))), nat.ptr(F.fr_to_limbs(F.fr_inv(n))), nat.ptr(out)))
     return out
 
 

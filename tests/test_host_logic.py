@@ -3,7 +3,6 @@ field / group-law / digit-recoding code that the CUDA kernels share with the hos
 import ctypes as C
 import os
 import random
-import re
 
 import numpy as np
 import pytest
@@ -18,12 +17,50 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_cabi_exports_every_declared_symbol():
-    hdr = open(os.path.join(ROOT, "include", "ezkl_b200.h")).read()
-    names = re.findall(r"^\s*(?:int|void|uint64_t|const char\*)\s+(b200_\w+)\s*\(", hdr, flags=re.M)
-    assert len(names) >= 40
-    lib = nat.lib()
-    for nm in names:
-        assert hasattr(lib, nm), "libezkl_b200.so does not export %s" % nm
+    """Every prototype of include/ezkl_b200.h (and of the test hooks' csrc/debug.h) is exported, with the argtypes / restype read from it."""
+    for load, header in ((nat.lib, nat.HEADER), (nat.dbg_lib, nat.DBG_HEADER)):
+        lib, decls = load(), nat.declarations(header)
+        assert len(decls) >= 13
+        for name, (argtypes, restype) in decls.items():
+            assert hasattr(lib, name), "%s does not export %s" % (lib._name, name)
+            fn = getattr(lib, name)
+            assert fn.argtypes == argtypes and fn.restype is restype, name
+
+
+def test_cabi_signatures_follow_the_header_types():
+    """Pointers are c_void_p; int, uint32_t, uint64_t and size_t keep their C width; every declared function is typed."""
+    prod, dbg = nat.declarations(nat.HEADER), nat.declarations(nat.DBG_HEADER)
+    assert (len(prod), len(dbg)) == (66, 13)
+    for decls in (prod, dbg):
+        for name, (argtypes, restype) in decls.items():
+            assert set(argtypes) <= {C.c_void_p, C.c_int, C.c_uint32, C.c_uint64, C.c_size_t}, name
+            assert restype in (C.c_int, C.c_uint64, C.c_char_p, None), name
+    assert prod["b200_last_error"] == ([], C.c_char_p) and prod["b200_launch_count"] == ([], C.c_uint64)
+    assert prod["b200_shutdown"] == ([], None) and prod["b200_init"] == ([C.c_int], C.c_int)
+    assert prod["b200_msm"] == ([C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p], C.c_int)
+    assert prod["b200_fft"] == ([C.c_void_p, C.c_uint32, C.c_void_p], C.c_int)
+    assert prod["b200_ntt_dev"] == ([C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_int, C.c_void_p,
+                                     C.c_int, C.c_void_p, C.c_size_t, C.c_void_p], C.c_int)
+    assert dbg["b200_debug_msm_pick_levels"] == ([C.c_size_t, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p], C.c_int)
+    assert dbg["b200_debug_ntt_plan_host"] == ([C.c_uint32, C.c_int, C.c_int, C.c_void_p], C.c_int)
+
+
+def test_cabi_rejects_untyped_declarations(tmp_path):
+    """A parameter or return type outside the mapping, or a missing header, is an error at load, never an unchecked call."""
+    h = tmp_path / "h.h"
+    h.write_text("#include <stdint.h>\n/* int b200_commented(double d); */\nint b200_ok(size_t n, const void* p); // void b200_x(float f);\n")
+    assert nat.declarations(str(h)) == {"b200_ok": ([C.c_size_t, C.c_void_p], C.c_int)}
+    for decl in ("int b200_x(float f);", "float b200_x(int a);", "int b200_x(struct s v);", "int b200_x(int);"):
+        h.write_text("#include <stdint.h>\n" + decl + "\n")
+        with pytest.raises(nat.B200Error):
+            nat.declarations(str(h))
+    with pytest.raises(nat.B200Error):
+        nat.declarations(str(tmp_path / "missing.h"))
+
+
+def test_cabi_call_with_a_missing_argument_raises_before_the_library():
+    with pytest.raises(TypeError):
+        nat.lib().b200_poly_op(0, None)
 
 
 def test_no_cpu_fallback_without_device():

@@ -65,6 +65,16 @@ def test_pick_levels_properties():
     assert pick_levels(1 << 26, 20, DEFAULT_BUDGET) == (4, 4)
 
 
+def test_bare_int_above_2_32_reaches_a_size_t_intact():
+    """The declared argtypes pass a plain Python int at the full width of size_t; untyped, ctypes passes it as a 32-bit int.  The budget
+    is chosen so that cutting n to 5, the budget to 4096, or both, each gives a different level count than the intact call."""
+    n, budget = (1 << 33) + 5, (3 << 40) + 4096
+    s, L = C.c_int(0), C.c_int(0)
+    nat.check(nat.dbg_lib().b200_debug_msm_pick_levels(n, 16, budget, C.byref(s), C.byref(L)))
+    assert (s.value, L.value) == expected_levels(n, 16, budget) == (3, 6)
+    assert (3, 6) not in {expected_levels(5, 16, budget), expected_levels(n, 16, 4096), expected_levels(5, 16, 4096)}
+
+
 @pytest.mark.parametrize("c", [4, 7, 10, 13, 16, 20, 24])
 def test_digit_slots(c):
     """(level, bucket set, bucket, sign) of every digit, for each windows-per-level count: sum_r 2^(c r) sum_j 2^(c s j) d_(js+r) == x,
