@@ -82,8 +82,7 @@ struct Ctx {
     cudaStream_t stream = nullptr;
     MsmWorkspace msm_ws;
     PolyWorkspace poly_ws;
-    QuotientWorkspace quot_ws;
-    StagingRing ring;
+    StagingRing ring;                            // parameter blobs of every kernel launched from this context
     DevBuf stage_a, stage_b, stage_c, small;
     // pinned bounce buffers for large pageable <-> device copies (two slots, pipelined against the DMA engine)
     uint8_t* bounce[2] = {nullptr, nullptr};
@@ -94,10 +93,10 @@ struct Ctx {
     bool has_last = false;
     void release() {
         cudaSetDevice(dev);
-        DevBuf* bufs[] = {&msm_ws.counts, &msm_ws.offs, &msm_ws.ents, &msm_ws.subs, &msm_ws.sums, &msm_ws.misc, &msm_ws.tile_counts, &poly_ws.scratch, &quot_ws.prog,
+        DevBuf* bufs[] = {&msm_ws.counts, &msm_ws.offs, &msm_ws.ents, &msm_ws.subs, &msm_ws.sums, &msm_ws.misc, &msm_ws.tile_counts, &poly_ws.scratch,
                           &stage_a, &stage_b, &stage_c, &small};
         for (DevBuf* b : bufs) b->release();
-        ring.release(); poly_ws.ring.release(); quot_ws.ring.release();
+        ring.release();
         for (int i = 0; i < 2; ++i) { if (bounce[i]) cudaFreeHost(bounce[i]); if (bounce_ev[i]) cudaEventDestroy(bounce_ev[i]); bounce[i] = nullptr; bounce_ev[i] = nullptr; }
         if (last_ev) cudaEventDestroy(last_ev);
         if (stream) cudaStreamDestroy(stream);
@@ -579,7 +578,9 @@ int b200_dev_alloc_on(int slot, void** d_ptr, size_t bytes) {
 int b200_dev_free(void* d_ptr) { B200_CUDA(cudaFree(d_ptr)); return 0; }
 int b200_dev_upload(void* d_dst, const void* h_src, size_t bytes) {
     B200_ENTER(c, d_dst);
-    B200_CUDA(cudaMemcpyAsync(d_dst, h_src, bytes, cudaMemcpyHostToDevice, c->stream));
+    if (bytes == 0) return 0;
+    B200_CHECK(d_dst && h_src, -1, "dev_upload: null pointer");
+    if (int rc = h2d_one(c, d_dst, h_src, bytes, c->stream)) return rc;
     B200_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -591,9 +592,9 @@ int b200_dev_upload_async(void* d_dst, const void* h_src, size_t bytes, void* st
 }
 int b200_dev_download(void* h_dst, const void* d_src, size_t bytes) {
     B200_ENTER(c, d_src);
-    B200_CUDA(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, c->stream));
-    B200_CUDA(cudaStreamSynchronize(c->stream));
-    return 0;
+    if (bytes == 0) return 0;
+    B200_CHECK(h_dst && d_src, -1, "dev_download: null pointer");
+    return d2h_one(c, h_dst, d_src, bytes, c->stream);
 }
 int b200_host_alloc(void** h_ptr, size_t bytes) { B200_CUDA(cudaMallocHost(h_ptr, bytes)); return 0; }
 int b200_host_free(void* h_ptr) { B200_CUDA(cudaFreeHost(h_ptr)); return 0; }
@@ -947,7 +948,7 @@ static int ntt_host(const b200_fr* const* src, b200_fr* const* dst, size_t batch
             if (cs->stage_a.ensure(sizeof(Fr) * slice) || cs->stage_b.ensure(sizeof(Fr) * slice)) return -2;
             wcs[s] = cs; sl_src[s] = cs->stage_a.as<Fr>(); sl_tmp[s] = cs->stage_b.as<Fr>(); sl_dst[s] = cs->stage_a.as<Fr>();
             const size_t lo = slice * s, hi = lo + slice < n_in ? lo + slice : n_in;
-            if (hi > lo) B200_CUDA(cudaMemcpyAsync(sl_src[s], src[0] + lo, sizeof(Fr) * (hi - lo), cudaMemcpyHostToDevice, cs->stream));
+            if (hi > lo) { if (int r = h2d_one(cs, sl_src[s], src[0] + lo, sizeof(Fr) * (hi - lo), cs->stream)) return r; }
             B200_CUDA(cudaStreamSynchronize(cs->stream));
             return 0;
         });
@@ -957,9 +958,7 @@ static int ntt_host(const b200_fr* const* src, b200_fr* const* dst, size_t batch
         return run_on_slots(nd, [&](int s) -> int {
             Ctx* cs = wcs[s];
             DevGuard dg(cs);
-            B200_CUDA(cudaMemcpyAsync(dst[0] + slice * s, sl_dst[s], sizeof(Fr) * slice, cudaMemcpyDeviceToHost, cs->stream));
-            B200_CUDA(cudaStreamSynchronize(cs->stream));
-            return 0;
+            return d2h_one(cs, dst[0] + slice * s, sl_dst[s], sizeof(Fr) * slice, cs->stream);
         });
     }
     return ntt_host_on(c, src, dst, batch, n_in, log_n, omega, pre, post);
@@ -1028,7 +1027,7 @@ static int lincomb_on(Ctx* c, cudaStream_t st, const void* const* d_polys, const
     B200_CHECK(d_out && (count == 0 || (d_polys && scalars)), -1, "poly_lincomb: null pointer");
     std::vector<Fr> sv(count);
     if (count) memcpy(sv.data(), scalars, sizeof(Fr) * count);
-    return poly_lincomb(reinterpret_cast<const Fr* const*>(d_polys), sv.data(), count, reinterpret_cast<Fr*>(d_out), n, c->poly_ws, st);
+    return poly_lincomb(reinterpret_cast<const Fr* const*>(d_polys), sv.data(), count, reinterpret_cast<Fr*>(d_out), n, c->ring, st);
 }
 int b200_poly_lincomb_dev(const void* const* d_polys, const b200_fr* scalars, size_t count, size_t n, void* d_out, void* stream) {
     B200_ENTER(c, d_out); StreamScope ss(c, stream);
@@ -1053,13 +1052,7 @@ int b200_poly_lincomb(const b200_fr* const* polys, const b200_fr* scalars, size_
 }
 static int scale_cycle_on(Ctx* c, cudaStream_t st, void* d_a, size_t n, const b200_fr* consts, uint32_t period) {
     B200_CHECK(d_a && consts && period > 0 && period <= 1024, -1, "poly_scale_cycle: bad argument");
-    const Fr* d_consts = reinterpret_cast<const Fr*>(c->ring.push(consts, sizeof(Fr) * period, st));
-    if (!d_consts) {
-        if (c->small.ensure(sizeof(Fr) * period)) return -2;
-        B200_CUDA(cudaMemcpyAsync(c->small.p, consts, sizeof(Fr) * period, cudaMemcpyHostToDevice, st));
-        d_consts = c->small.as<Fr>();
-    }
-    return poly_scale_cycle(reinterpret_cast<const Fr*>(d_a), d_consts, period, reinterpret_cast<Fr*>(d_a), n, st);
+    return poly_scale_cycle(reinterpret_cast<const Fr*>(d_a), reinterpret_cast<const Fr*>(consts), period, reinterpret_cast<Fr*>(d_a), n, c->ring, st);
 }
 int b200_poly_scale_cycle_dev(void* d_a, size_t n, const b200_fr* consts, uint32_t period, void* stream) {
     B200_ENTER(c, d_a); StreamScope ss(c, stream);
@@ -1080,7 +1073,7 @@ static int eval_batch_on(Ctx* c, cudaStream_t st, const void* d_polys, size_t st
     if (batch == 0) return 0;
     std::vector<Fr> xv(batch);
     memcpy(xv.data(), x, sizeof(Fr) * batch);
-    return poly_eval(reinterpret_cast<const Fr*>(d_polys), stride, n, xv.data(), reinterpret_cast<Fr*>(d_out), (int)batch, c->poly_ws, st);
+    return poly_eval(reinterpret_cast<const Fr*>(d_polys), stride, n, xv.data(), reinterpret_cast<Fr*>(d_out), (int)batch, c->poly_ws, c->ring, st);
 }
 int b200_poly_eval_batch_dev(const void* d_polys, size_t stride, size_t n, const b200_fr* x, size_t batch, void* d_out, void* stream) {
     B200_ENTER(c, d_polys); StreamScope ss(c, stream);
@@ -1129,7 +1122,7 @@ static int prefix_scan_on(Ctx* c, cudaStream_t st, int product, const void* d_a,
     if (batch == 0) return 0;
     std::vector<Fr> iv(batch);
     memcpy(iv.data(), inits, sizeof(Fr) * batch);
-    return poly_prefix_scan(product != 0, reinterpret_cast<const Fr*>(d_a), a_stride, n, iv.data(), reinterpret_cast<Fr*>(d_out), out_stride, (int)batch, c->poly_ws, st);
+    return poly_prefix_scan(product != 0, reinterpret_cast<const Fr*>(d_a), a_stride, n, iv.data(), reinterpret_cast<Fr*>(d_out), out_stride, (int)batch, c->poly_ws, c->ring, st);
 }
 int b200_prefix_scan_dev(int product, const void* d_a, size_t n, const b200_fr* init, void* d_out, void* stream) {
     B200_ENTER(c, d_a); StreamScope ss(c, stream);
@@ -1154,7 +1147,7 @@ static int kate_division_on(Ctx* c, cudaStream_t st, const void* d_a, size_t n, 
     // q[e] is computed from a[e + 1 ..]: a thread's stores would overwrite the coefficient its neighbour still has to read
     B200_CHECK(d_q != d_a, -1, "kate_division: q must not alias a (the quotient cannot be computed in place)");
     const Fr bv = as_fr(b);
-    return poly_kate_division(reinterpret_cast<const Fr*>(d_a), n, &bv, reinterpret_cast<Fr*>(d_q), c->poly_ws, st);
+    return poly_kate_division(reinterpret_cast<const Fr*>(d_a), n, &bv, reinterpret_cast<Fr*>(d_q), c->poly_ws, c->ring, st);
 }
 int b200_kate_division_dev(const void* d_a, size_t n, const b200_fr* b, void* d_q, void* stream) {
     B200_ENTER(c, d_a); StreamScope ss(c, stream);
@@ -1176,16 +1169,9 @@ int b200_kate_division(const b200_fr* a, size_t n, const b200_fr* b, b200_fr* q)
 static int lookup_multiplicities_on(Ctx* c, cudaStream_t st, const void* d_table, size_t n_table, const void* const* d_inputs, size_t n_inputs, size_t n_rows, void* d_m,
                                     uint64_t* missing) {
     B200_CHECK(d_table && d_m && d_inputs && n_inputs >= 1, -1, "lookup_multiplicities: null pointer");
-    const void* d_ptrs = c->ring.push(d_inputs, sizeof(void*) * n_inputs, st);
-    if (!d_ptrs) {
-        if (c->small.ensure(sizeof(void*) * n_inputs)) return -2;
-        B200_CUDA(cudaMemcpyAsync(c->small.p, d_inputs, sizeof(void*) * n_inputs, cudaMemcpyHostToDevice, st));
-        B200_CUDA(cudaStreamSynchronize(st));
-        d_ptrs = c->small.p;
-    }
     unsigned long long* d_missing = nullptr;
-    if (int rc = lookup_multiplicities_run(reinterpret_cast<const Fr*>(d_table), n_table, reinterpret_cast<const Fr* const*>(d_ptrs), n_inputs, n_rows,
-                                           reinterpret_cast<Fr*>(d_m), c->msm_ws.misc, &d_missing, st)) return rc;
+    if (int rc = lookup_multiplicities_run(reinterpret_cast<const Fr*>(d_table), n_table, reinterpret_cast<const Fr* const*>(d_inputs), n_inputs, n_rows,
+                                           reinterpret_cast<Fr*>(d_m), c->msm_ws.misc, c->ring, &d_missing, st)) return rc;
     if (missing) {
         unsigned long long h = 0;
         B200_CUDA(cudaMemcpyAsync(&h, d_missing, sizeof h, cudaMemcpyDeviceToHost, st));
@@ -1234,7 +1220,7 @@ static int quotient_eval_on(Ctx* c, cudaStream_t st, const void* const* d_column
         ql[i].offset = (uint32_t)(((off % (int64_t)N) + (int64_t)N) % (int64_t)N);
     }
     return quotient_eval_run(reinterpret_cast<const Fr* const*>(d_columns), n_columns, ext_k, ql.data(), n_loads, reinterpret_cast<const Fr*>(constants), n_constants,
-                             reinterpret_cast<const QInstr*>(program), n_instr, reinterpret_cast<Fr*>(d_out), c->quot_ws, st);
+                             reinterpret_cast<const QInstr*>(program), n_instr, reinterpret_cast<Fr*>(d_out), c->ring, st);
 }
 int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
                            const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out, void* stream) {

@@ -51,35 +51,55 @@ struct DevBuf {
     template <class T> T* as() { return reinterpret_cast<T*>(p); }
 };
 
-// Small host->device parameter blobs (programs, pointer tables, per-call constants) without a stream synchronisation:
-// the blob is copied into a slot of a pinned ring and an async H2D copy into the matching slot of a device ring is enqueued
-// on the caller's stream, followed by an event.  A slot is reused only after its own event has completed (a host-side wait
-// on that one event — never a device-wide synchronisation), so neither the pinned source nor the device copy can be
-// overwritten while a kernel may still read it.  Not capturable in a CUDA graph (a replay would re-read the pinned slot).
+// Host->device parameter blobs (programs, pointer tables, per-call constants): one ring per (thread, device) context, pushed
+// only by the kernel files, at most one blob per launch sequence.  push() stages `bytes` from `src`, sets *d_out to the device
+// copy and returns 0; when it returns, the host source may be reused.
+//   * A blob of at most SLOT bytes goes without a stream synchronisation: it is copied into a slot of a pinned ring and an async
+//     H2D copy into the matching slot of a device ring is enqueued on the caller's stream, followed by an event.  A slot is reused
+//     only after its own event has completed (a host-side wait on that one event — never a device-wide synchronisation), so
+//     neither the pinned source nor the device copy can be overwritten while a kernel may still read it.
+//   * A larger blob, or any blob while the pinned ring cannot be allocated, is copied into `overflow` and the stream is
+//     synchronised.  An overflow blob is valid until the next push on this ring: the caller enqueues the kernels that read it
+//     before it pushes again, so the next overflow copy is ordered after them.
+//   * A failing CUDA call returns -2 with the error set.
+// Not capturable in a CUDA graph (a replay would re-read the pinned slot).
 struct StagingRing {
     static constexpr size_t SLOT = (size_t)256 << 10;
-    static constexpr int NSLOT = 32;
+    static constexpr int NSLOT = 96;
     uint8_t* h = nullptr;
     uint8_t* d = nullptr;
     cudaEvent_t ev[NSLOT] = {};
     bool used[NSLOT] = {};
     int head = 0;
-    void* push(const void* src, size_t bytes, cudaStream_t st) {
-        if (bytes > SLOT) return nullptr;                          // caller falls back to its synchronous path
-        if (!h) {
-            if (cudaMallocHost((void**)&h, SLOT * NSLOT) != cudaSuccess || cudaMalloc((void**)&d, SLOT * NSLOT) != cudaSuccess) { cudaGetLastError(); release(); return nullptr; }
-            for (int i = 0; i < NSLOT; ++i) if (cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) != cudaSuccess) { release(); return nullptr; }
+    DevBuf overflow;
+    int push(const void* src, size_t bytes, cudaStream_t st, const void** d_out) {
+        if (bytes <= SLOT && !h && !alloc_ring()) { cudaGetLastError(); release_ring(); }
+        if (bytes > SLOT || !h) {
+            if (overflow.ensure(bytes)) return -2;
+            B200_CUDA(cudaMemcpyAsync(overflow.p, src, bytes, cudaMemcpyHostToDevice, st));
+            B200_CUDA(cudaStreamSynchronize(st));
+            *d_out = overflow.p;
+            return 0;
         }
         const int s = head;
         head = (head + 1) % NSLOT;
-        if (used[s] && cudaEventSynchronize(ev[s]) != cudaSuccess) return nullptr;
+        if (used[s]) B200_CUDA(cudaEventSynchronize(ev[s]));
         memcpy(h + s * SLOT, src, bytes);
-        if (cudaMemcpyAsync(d + s * SLOT, h + s * SLOT, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) return nullptr;
-        if (cudaEventRecord(ev[s], st) != cudaSuccess) return nullptr;
+        B200_CUDA(cudaMemcpyAsync(d + s * SLOT, h + s * SLOT, bytes, cudaMemcpyHostToDevice, st));
+        B200_CUDA(cudaEventRecord(ev[s], st));
         used[s] = true;
-        return d + s * SLOT;
+        *d_out = d + s * SLOT;
+        return 0;
     }
-    void release() {
+    void release() { release_ring(); overflow.release(); }
+private:
+    bool alloc_ring() {
+        if (cudaMallocHost((void**)&h, SLOT * NSLOT) != cudaSuccess) { h = nullptr; return false; }
+        if (cudaMalloc((void**)&d, SLOT * NSLOT) != cudaSuccess) { d = nullptr; return false; }
+        for (int i = 0; i < NSLOT; ++i) if (cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) != cudaSuccess) { ev[i] = nullptr; return false; }
+        return true;
+    }
+    void release_ring() {
         if (h) cudaFreeHost(h);
         if (d) cudaFree(d);
         for (int i = 0; i < NSLOT; ++i) { if (ev[i]) cudaEventDestroy(ev[i]); ev[i] = nullptr; used[i] = false; }

@@ -63,10 +63,13 @@ __global__ void __launch_bounds__(256) k_lk_finish(const uint32_t* __restrict__ 
     fp_store(m + i, counts[i] ? fp_to_mont(c) : c);
 }
 
-// d_inputs: DEVICE array of n_inputs device pointers.  scratch layout: [slots 2^s][counts n_table][missing u64]
-int lookup_multiplicities_run(const Fr* d_table, size_t n_table, const Fr* const* d_inputs, size_t n_inputs, size_t n_rows, Fr* d_m, DevBuf& scratch,
+// scratch layout: [slots 2^s][counts n_table][missing u64]
+int lookup_multiplicities_run(const Fr* d_table, size_t n_table, const Fr* const* h_inputs, size_t n_inputs, size_t n_rows, Fr* d_m, DevBuf& scratch, StagingRing& ring,
                               unsigned long long** d_missing_out, cudaStream_t st) {
     B200_CHECK(n_table >= 1 && n_table < (1u << 30) && n_rows < (1u << 31) && n_inputs >= 1 && n_inputs <= 65535, -1, "lookup_multiplicities: sizes out of range");
+    const void* staged;
+    if (int rc = ring.push(h_inputs, sizeof(void*) * n_inputs, st, &staged)) return rc;
+    const Fr* const* d_inputs = reinterpret_cast<const Fr* const*>(staged);
     uint32_t cap = 64;
     while (cap < 2 * n_table) cap <<= 1;
     const size_t bytes = sizeof(uint32_t) * ((size_t)cap + n_table) + 16;

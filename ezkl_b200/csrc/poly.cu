@@ -51,27 +51,25 @@ int poly_binary(int op, const Fr* a, const Fr* b, const Fr* h_s, Fr* out, size_t
     B200_CUDA(cudaGetLastError());
     return 0;
 }
-int poly_lincomb(const Fr* const* h_polys /*device addresses*/, const Fr* h_scalars, size_t count, Fr* out, size_t n, PolyWorkspace& ws, cudaStream_t st) {
+int poly_lincomb(const Fr* const* h_polys /*device addresses*/, const Fr* h_scalars, size_t count, Fr* out, size_t n, StagingRing& ring, cudaStream_t st) {
     if (n == 0) return 0;
     B200_CHECK(count < (1u << 24), -1, "poly_lincomb: too many terms");
     const size_t o_s = (sizeof(void*) * count + 31) & ~(size_t)31, total = o_s + sizeof(Fr) * count + 32;
     std::vector<uint8_t> blob(total, 0);
     if (count) { memcpy(blob.data(), h_polys, sizeof(void*) * count); memcpy(blob.data() + o_s, h_scalars, sizeof(Fr) * count); }
-    uint8_t* d = reinterpret_cast<uint8_t*>(ws.ring.push(blob.data(), total, st));
-    if (!d) {
-        if (ws.scratch.ensure(total)) return -2;
-        B200_CUDA(cudaMemcpyAsync(ws.scratch.p, blob.data(), total, cudaMemcpyHostToDevice, st));
-        B200_CUDA(cudaStreamSynchronize(st));
-        d = ws.scratch.as<uint8_t>();
-    }
+    const void* staged;
+    if (int rc = ring.push(blob.data(), total, st, &staged)) return rc;
+    const uint8_t* d = reinterpret_cast<const uint8_t*>(staged);
     k_poly_lincomb<<<ew_grid(n), 256, 0, st>>>(reinterpret_cast<const Fr* const*>(d), reinterpret_cast<const Fr*>(d + o_s), (uint32_t)count, out, n); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
-int poly_scale_cycle(const Fr* a, const Fr* d_consts, uint32_t period, Fr* out, size_t n, cudaStream_t st) {
+int poly_scale_cycle(const Fr* a, const Fr* h_consts, uint32_t period, Fr* out, size_t n, StagingRing& ring, cudaStream_t st) {
     if (n == 0) return 0;
     B200_CHECK(period > 0, -1, "poly_scale_cycle: period 0");
-    k_poly_scale_cycle<<<ew_grid(n), 256, 0, st>>>(a, d_consts, period, out, n); count_launch();
+    const void* d_consts;
+    if (int rc = ring.push(h_consts, sizeof(Fr) * period, st, &d_consts)) return rc;
+    k_poly_scale_cycle<<<ew_grid(n), 256, 0, st>>>(a, reinterpret_cast<const Fr*>(d_consts), period, out, n); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
@@ -176,42 +174,38 @@ __global__ void __launch_bounds__(TB) k_wscan_apply(const Fr* __restrict__ a, si
 
 static unsigned carry_threads(uint32_t nblk) { unsigned t = 32; while (t < nblk && t < 1024) t <<= 1; return t; }
 
-static int upload_wargs(const Fr* h_x, int batch, PolyWorkspace& ws, size_t extra_bytes, WArgs** d_w, uint8_t** d_extra, cudaStream_t st) {
-    const size_t wbytes = sizeof(WArgs) * batch;
+static int upload_wargs(const Fr* h_x, int batch, StagingRing& ring, const WArgs** d_w, cudaStream_t st) {
     std::vector<WArgs> hw(batch);
     for (int p = 0; p < batch; ++p) { hw[p].x = h_x[p]; hw[p].xc = fp_pow_u64(h_x[p], CHUNK); hw[p].xt = fp_pow_u64(h_x[p], TILE); }
-    if (ws.scratch.ensure(wbytes + 256 + extra_bytes)) return -2;
-    *d_extra = ws.scratch.as<uint8_t>() + ((wbytes + 255) & ~(size_t)255);
-    *d_w = reinterpret_cast<WArgs*>(ws.ring.push(hw.data(), wbytes, st));
-    if (!*d_w) {
-        *d_w = ws.scratch.as<WArgs>();
-        B200_CUDA(cudaMemcpyAsync(*d_w, hw.data(), wbytes, cudaMemcpyHostToDevice, st));
-        B200_CUDA(cudaStreamSynchronize(st));   // hw is a stack temporary
-    }
+    const void* staged;
+    if (int rc = ring.push(hw.data(), sizeof(WArgs) * batch, st, &staged)) return rc;
+    *d_w = reinterpret_cast<const WArgs*>(staged);
     return 0;
 }
 
-int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_out, int batch, PolyWorkspace& ws, cudaStream_t st) {
+int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_out, int batch, PolyWorkspace& ws, StagingRing& ring, cudaStream_t st) {
     B200_CHECK(batch > 0 && batch <= 65535, -1, "poly_eval: batch %d out of range", batch);
     if (n == 0) { B200_CUDA(cudaMemsetAsync(d_out, 0, sizeof(Fr) * batch, st)); return 0; }
     const uint32_t nblk = div_up(n, TILE);
-    WArgs* d_w; uint8_t* extra;
-    if (int rc = upload_wargs(h_x, batch, ws, sizeof(Fr) * (size_t)nblk * batch, &d_w, &extra, st)) return rc;
-    Fr* blk_val = reinterpret_cast<Fr*>(extra);
+    if (ws.scratch.ensure(sizeof(Fr) * (size_t)nblk * batch)) return -2;
+    const WArgs* d_w;
+    if (int rc = upload_wargs(h_x, batch, ring, &d_w, st)) return rc;
+    Fr* blk_val = ws.scratch.as<Fr>();
     k_wscan_block_values<<<dim3(nblk, batch), TB, 0, st>>>(coeffs, stride, n, d_w, blk_val, nblk); count_launch();
     k_wscan_carries<<<batch, carry_threads(nblk), 0, st>>>(blk_val, nblk, d_w, nullptr, d_out); count_launch();
     B200_CUDA(cudaGetLastError());
     return 0;
 }
 
-int poly_kate_division(const Fr* a, size_t n, const Fr* h_b, Fr* q, PolyWorkspace& ws, cudaStream_t st) {
+int poly_kate_division(const Fr* a, size_t n, const Fr* h_b, Fr* q, PolyWorkspace& ws, StagingRing& ring, cudaStream_t st) {
     B200_CHECK(n >= 1, -1, "kate_division: empty polynomial");
     if (n == 1) return 0;
     const size_t m = n - 1;
     const uint32_t nblk = div_up(m, TILE);
-    WArgs* d_w; uint8_t* extra;
-    if (int rc = upload_wargs(h_b, 1, ws, sizeof(Fr) * (size_t)nblk * 2, &d_w, &extra, st)) return rc;
-    Fr* blk_val = reinterpret_cast<Fr*>(extra);
+    if (ws.scratch.ensure(sizeof(Fr) * (size_t)nblk * 2)) return -2;
+    const WArgs* d_w;
+    if (int rc = upload_wargs(h_b, 1, ring, &d_w, st)) return rc;
+    Fr* blk_val = ws.scratch.as<Fr>();
     Fr* carry = blk_val + nblk;
     k_wscan_block_values<<<dim3(nblk, 1), TB, 0, st>>>(a + 1, 0, m, d_w, blk_val, nblk); count_launch();
     k_wscan_carries<<<1, carry_threads(nblk), 0, st>>>(blk_val, nblk, d_w, carry, nullptr); count_launch();
@@ -268,28 +262,25 @@ __global__ void __launch_bounds__(TB) k_scan_apply(const Fr* __restrict__ a_all,
 }
 
 // `batch` independent columns a[p * a_stride ..] -> out[p * out_stride ..], one initial value each (h_inits: host array)
-int poly_prefix_scan(bool product, const Fr* a, size_t a_stride, size_t n, const Fr* h_inits, Fr* out, size_t out_stride, int batch, PolyWorkspace& ws, cudaStream_t st) {
+int poly_prefix_scan(bool product, const Fr* a, size_t a_stride, size_t n, const Fr* h_inits, Fr* out, size_t out_stride, int batch, PolyWorkspace& ws, StagingRing& ring,
+                     cudaStream_t st) {
     if (n == 0 || batch == 0) return 0;
     B200_CHECK(batch > 0 && batch <= 65535, -1, "prefix_scan: batch %d out of range", batch);
     const uint32_t nblk = div_up(n, TILE);
-    if (ws.scratch.ensure(sizeof(Fr) * ((size_t)nblk * 2 + 1) * batch)) return -2;
+    if (ws.scratch.ensure(sizeof(Fr) * (size_t)nblk * 2 * batch)) return -2;
     Fr* blk_tot = ws.scratch.as<Fr>();
     Fr* blk_pre = blk_tot + (size_t)nblk * batch;
-    Fr* d_init = blk_pre + (size_t)nblk * batch;
-    const Fr* staged = reinterpret_cast<const Fr*>(ws.ring.push(h_inits, sizeof(Fr) * batch, st));
-    if (!staged) {
-        B200_CUDA(cudaMemcpyAsync(d_init, h_inits, sizeof(Fr) * batch, cudaMemcpyHostToDevice, st));
-        B200_CUDA(cudaStreamSynchronize(st));       // h_inits is the caller's temporary
-        staged = d_init;
-    }
+    const void* staged;
+    if (int rc = ring.push(h_inits, sizeof(Fr) * batch, st, &staged)) return rc;
+    const Fr* d_inits = reinterpret_cast<const Fr*>(staged);
     const dim3 grid(nblk, batch);
     if (product) {
         k_scan_block_totals<true><<<grid, TB, 0, st>>>(a, a_stride, n, blk_tot, nblk); count_launch();
-        k_scan_block_prefixes<true><<<batch, 1024, 0, st>>>(blk_tot, nblk, staged, blk_pre); count_launch();
+        k_scan_block_prefixes<true><<<batch, 1024, 0, st>>>(blk_tot, nblk, d_inits, blk_pre); count_launch();
         k_scan_apply<true><<<grid, TB, 0, st>>>(a, a_stride, n, blk_pre, nblk, out, out_stride); count_launch();
     } else {
         k_scan_block_totals<false><<<grid, TB, 0, st>>>(a, a_stride, n, blk_tot, nblk); count_launch();
-        k_scan_block_prefixes<false><<<batch, 1024, 0, st>>>(blk_tot, nblk, staged, blk_pre); count_launch();
+        k_scan_block_prefixes<false><<<batch, 1024, 0, st>>>(blk_tot, nblk, d_inits, blk_pre); count_launch();
         k_scan_apply<false><<<grid, TB, 0, st>>>(a, a_stride, n, blk_pre, nblk, out, out_stride); count_launch();
     }
     B200_CUDA(cudaGetLastError());

@@ -7,25 +7,28 @@ namespace b200 {
 
 enum PolyOp { POLY_ADD = 0, POLY_SUB = 1, POLY_MUL = 2, POLY_SCALE = 3, POLY_AXPY = 4 };
 
-struct PolyWorkspace { DevBuf scratch; StagingRing ring; };
+struct PolyWorkspace { DevBuf scratch; };
 
 // out[i] = a[i] (+|-|*) b[i]  |  a[i]*s  |  a[i] + s*b[i]        (all device pointers; out may alias a or b)
 int poly_binary(int op, const Fr* a, const Fr* b, const Fr* h_s, Fr* out, size_t n, cudaStream_t st);   // h_s: host scalar
+// The host arrays (h_*) below are staged through `ring` (common.cuh: StagingRing) and may be reused when the call returns.
 // out[i] = sum_j scalars[j] * polys[j][i]; h_polys = host array of device addresses, h_scalars = host scalars
-int poly_lincomb(const Fr* const* h_polys, const Fr* h_scalars, size_t count, Fr* out, size_t n, PolyWorkspace& ws, cudaStream_t st);
-// out[i] = a[i] * consts[i mod period]   (distribute_powers_zeta: period 3; divide_by_vanishing_poly: period 2^(ext_k-k))
-int poly_scale_cycle(const Fr* a, const Fr* d_consts, uint32_t period, Fr* out, size_t n, cudaStream_t st);
+int poly_lincomb(const Fr* const* h_polys, const Fr* h_scalars, size_t count, Fr* out, size_t n, StagingRing& ring, cudaStream_t st);
+// out[i] = a[i] * consts[i mod period]   (distribute_powers_zeta: period 3; divide_by_vanishing_poly: period 2^(ext_k-k)); h_consts host array
+int poly_scale_cycle(const Fr* a, const Fr* h_consts, uint32_t period, Fr* out, size_t n, StagingRing& ring, cudaStream_t st);
 // out[p] = sum_i coeffs[p*stride + i] * x[p]^i   for p < batch (eval_polynomial); h_x host array, d_out device array
-int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_out, int batch, PolyWorkspace& ws, cudaStream_t st);
+int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_out, int batch, PolyWorkspace& ws, StagingRing& ring, cudaStream_t st);
 // in place a[i] <- a[i]^-1 (zeros stay zero)  (ff::BatchInvert)
 int poly_batch_invert(Fr* a, size_t n, PolyWorkspace& ws, cudaStream_t st);
 // exclusive running product / sum per column: out[p][0] = inits[p], out[p][i+1] = out[p][i] (op) a[p][i], p < batch
-int poly_prefix_scan(bool product, const Fr* a, size_t a_stride, size_t n, const Fr* h_inits, Fr* out, size_t out_stride, int batch, PolyWorkspace& ws, cudaStream_t st);
+int poly_prefix_scan(bool product, const Fr* a, size_t a_stride, size_t n, const Fr* h_inits, Fr* out, size_t out_stride, int batch, PolyWorkspace& ws, StagingRing& ring,
+                     cudaStream_t st);
 // quotient of a(X) by (X - b): q has n-1 coefficients (kate_division)
-int poly_kate_division(const Fr* a, size_t n, const Fr* h_b, Fr* q, PolyWorkspace& ws, cudaStream_t st);
+int poly_kate_division(const Fr* a, size_t n, const Fr* h_b, Fr* q, PolyWorkspace& ws, StagingRing& ring, cudaStream_t st);
 
 // mv-lookup multiplicities (lookup.cu): m[i] = number of input cells equal to table[i], counted on the first row holding each value
-int lookup_multiplicities_run(const Fr* d_table, size_t n_table, const Fr* const* d_inputs /*device array*/, size_t n_inputs, size_t n_rows, Fr* d_m, DevBuf& scratch,
+// h_inputs: host array of n_inputs device addresses
+int lookup_multiplicities_run(const Fr* d_table, size_t n_table, const Fr* const* h_inputs, size_t n_inputs, size_t n_rows, Fr* d_m, DevBuf& scratch, StagingRing& ring,
                               unsigned long long** d_missing_out, cudaStream_t st);
 
 }  // namespace b200

@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(128) k_quotient_eval(const uint4* __restrict__
 }
 
 int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k, const QLoad* h_loads, size_t n_loads, const Fr* h_consts, size_t n_consts,
-                      const QInstr* h_prog, size_t n_instr, Fr* d_out, QuotientWorkspace& ws, cudaStream_t st) {
+                      const QInstr* h_prog, size_t n_instr, Fr* d_out, StagingRing& ring, cudaStream_t st) {
     B200_CHECK(ext_k >= 1 && ext_k <= 28, -1, "quotient_eval: ext_k %u out of range", ext_k);
     B200_CHECK(n_instr < (1u << 24) && n_loads < (1u << 30) && n_consts < (1u << 30), -1, "quotient_eval: program too large");
     const uint32_t N = 1u << ext_k;
@@ -92,13 +92,8 @@ int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k
         memcpy(blob.data() + o_loads + sizeof(QLoadDev) * i, &l, sizeof l);
     }
     if (n_consts) memcpy(blob.data() + o_consts, h_consts, sizeof(Fr) * n_consts);
-    uint8_t* d = reinterpret_cast<uint8_t*>(ws.ring.push(blob.data(), total, st));
-    if (!d) {
-        if (ws.prog.ensure(total)) return -2;
-        B200_CUDA(cudaMemcpyAsync(ws.prog.p, blob.data(), total, cudaMemcpyHostToDevice, st));
-        B200_CUDA(cudaStreamSynchronize(st));      // blob is a stack temporary
-        d = ws.prog.as<uint8_t>();
-    }
+    const void* d;
+    if (int rc = ring.push(blob.data(), total, st, &d)) return rc;
     const uint32_t blob_u4 = (uint32_t)((total + 15) / 16);
     const size_t smem = (size_t)blob_u4 * 16;
     const dim3 grid(div_up(N, 128));

@@ -14,10 +14,9 @@ static constexpr uint32_t Q_NOSTORE = 0x80000000u;     // op_dst flag: the resul
 struct QInstr { uint32_t op_dst; uint32_t a, b, c; };   // op_dst = op | (dst_slot << 8) | NOSTORE;  MULADD: a * b + c
 struct QLoad { uint32_t column; uint32_t offset; };      // element offset already reduced mod 2^ext_k
 
-struct QuotientWorkspace { DevBuf prog; StagingRing ring; };
-
-// out[idx] = program(columns[c][(idx + offset) mod N], constants) for idx < N = 2^ext_k.  h_* are host arrays.
+// out[idx] = program(columns[c][(idx + offset) mod N], constants) for idx < N = 2^ext_k.  h_* are host arrays; the program is staged
+// through `ring` (common.cuh: StagingRing).
 int quotient_eval_run(const Fr* const* h_col_ptrs /*device addresses*/, size_t n_cols, uint32_t ext_k, const QLoad* h_loads, size_t n_loads,
-                      const Fr* h_consts, size_t n_consts, const QInstr* h_prog, size_t n_instr, Fr* d_out, QuotientWorkspace& ws, cudaStream_t st);
+                      const Fr* h_consts, size_t n_consts, const QInstr* h_prog, size_t n_instr, Fr* d_out, StagingRing& ring, cudaStream_t st);
 
 }  // namespace b200

@@ -216,6 +216,8 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
 int b200_dev_alloc(void** d_ptr, size_t bytes);
 int b200_dev_alloc_on(int device_slot, void** d_ptr, size_t bytes);   /* multi-device process: allocate on device `device_slot` */
 int b200_dev_free(void* d_ptr);
+/* synchronous: on return the bytes are on the device (upload) or in h_dst (download).  Pageable host memory is staged like every
+ * host-pointer entry point's columns; a null pointer with bytes > 0 is an argument error (-1) */
 int b200_dev_upload(void* d_dst, const void* h_src, size_t bytes);
 /* enqueue-only upload on `stream` (NULL = the calling thread's library stream); the host buffer must be pinned (b200_host_alloc)
  * and stay untouched until the stream reaches the copy: lets a resident-column shim overlap witness uploads with the first commits */

@@ -263,7 +263,9 @@ def test_scan_eval_kate_host_pointers(gpu, n):
 
 # ---- 2. batched and strided calls, in place ----------------------------------------------------------------------------------------------------
 @gpu_test
-@pytest.mark.parametrize("n,batch", [(5000, 1), (5000, 3), (5000, 7), ((1 << 22) + 4096 + 5, 3)])
+# batch 9000: 9000 scan initial values (32 B each) and 9000 evaluation parameter sets (96 B each) are both larger than one 256 KiB
+# slot of the parameter staging ring (StagingRing::SLOT), so both go through its overflow buffer
+@pytest.mark.parametrize("n,batch", [(5000, 1), (5000, 3), (5000, 7), ((1 << 22) + 4096 + 5, 3), (5, 9000)])
 def test_scan_and_eval_batched(gpu, n, batch):
     a_stride, out_stride = n + 3, n + 7
     cols = [orc.gen_scalars(n, seed=2000 + 10 * batch + p) for p in range(batch)]
@@ -345,6 +347,19 @@ def test_elementwise_grid_stride(gpu, size):
             exp = orc.poly_op("axpy", exp, pool[c], H.fr_wire(sum(H.fr_unwire(sc[j]) for j in range(c, count, 5))), THREADS)
         assert_same(got, exp, "lincomb of %d terms, n=%d" % (count, n), tile=256, chunk=1)
     del t_pool
+    # 7000 distinct columns, the windows [j, j + n) of one tensor: the pointer table and scalars, 40 B per term, are larger than one
+    # 256 KiB slot of the parameter staging ring (StagingRing::SLOT holds at most 6552 terms), so they go through its overflow buffer
+    if n <= 257:
+        count = 7000
+        window = orc.gen_scalars(count + n - 1, seed=3030)
+        sc = orc.gen_scalars(count, seed=3031)
+        t_window = up(window)
+        got = down(g_lincomb([t_window[j:j + n] for j in range(count)], sc, n))
+        exp = np.zeros((n, 4), np.uint64)
+        for j in range(count):
+            exp = orc.poly_op("axpy", exp, window[j:j + n], sc[j])
+        assert_same(got, exp, "lincomb of %d distinct columns, n=%d" % (count, n), tile=256, chunk=1)
+        del t_window
 
     # cyclic constants: the product with the constants repeated down the column
     for period in (1, 2, 3, 8, 1024):
@@ -414,7 +429,10 @@ def run_lookup(pool, table_ids, input_ids, n_rows, host=False, want_missing=True
     return got_m, got_missing, exp_m, exp_missing
 
 
-LOOKUP_SHAPES = [(1, 100, 1), (32, 1000, 2), (33, 1000, 2), (4096, 0, 1), (1 << 16, 1 << 16, 4), (1 << 12, (1 << 20) + 17, 3), (1 << 20, 1 << 20, 2)]
+# (64, 5, 32769): the table of 32769 input pointers (8 B each) is 8 B larger than one 256 KiB slot of the parameter staging ring
+# (StagingRing::SLOT), so it goes through the ring's overflow buffer
+LOOKUP_SHAPES = [(1, 100, 1), (32, 1000, 2), (33, 1000, 2), (4096, 0, 1), (1 << 16, 1 << 16, 4), (1 << 12, (1 << 20) + 17, 3), (1 << 20, 1 << 20, 2),
+                 (64, 5, 32769)]
 
 
 @gpu_test

@@ -309,6 +309,18 @@ def test_error_behaviour():
     out = np.zeros(12, np.uint64)
     assert L.b200_msm(C.c_uint64(987654), nat.ptr(a), C.c_size_t(2), nat.ptr(out)) == -1
     assert b"unknown bases handle" in L.b200_last_error()
+    # the synchronous upload / download helpers: a null pointer with bytes > 0 is an argument error, an empty copy is nothing to do
+    d = C.c_void_p()
+    nat.check(L.b200_dev_alloc(C.byref(d), C.c_size_t(a.nbytes)))
+    try:
+        assert L.b200_dev_upload(d, None, C.c_size_t(a.nbytes)) == -1
+        assert L.b200_dev_upload(None, nat.ptr(a), C.c_size_t(a.nbytes)) == -1
+        assert L.b200_dev_download(None, d, C.c_size_t(a.nbytes)) == -1
+        assert L.b200_dev_download(nat.ptr(a), None, C.c_size_t(a.nbytes)) == -1
+        assert b"null pointer" in L.b200_last_error()
+        assert L.b200_dev_upload(d, None, C.c_size_t(0)) == 0 and L.b200_dev_download(None, d, C.c_size_t(0)) == 0
+    finally:
+        nat.check(L.b200_dev_free(d))
 
 
 def test_cpp_host_mirror():
@@ -617,6 +629,15 @@ def test_host_entry_points_on_the_bounce_path():
     assert np.array_equal(h2.best_multiexp(col, hb), dev.normalize(dev.msm_batch(db, dev.from_host(col)))[0])
     hb.release()
     db.release()
+    # b200_dev_upload -> b200_dev_download of a pageable buffer: n Fr through the bounce slots, 3 Fr through the plain copy
+    import torch
+    for m in (n, 3):
+        src = orc.gen_scalars(m, seed=101)
+        t = torch.empty((m, 4), dtype=torch.int64, device="cuda")
+        nat.check(nat.lib().b200_dev_upload(nat.dev(t.data_ptr()), nat.ptr(src), C.c_size_t(src.nbytes)))
+        back = np.zeros_like(src)
+        nat.check(nat.lib().b200_dev_download(nat.ptr(back), nat.dev(t.data_ptr()), C.c_size_t(src.nbytes)))
+        assert np.array_equal(back, src) and np.array_equal(dev.to_host(t), src), "dev_upload / dev_download round trip of %d Fr" % m
 
 
 def test_launch_count_matches_the_profiler():
