@@ -200,7 +200,9 @@ static inline Fr as_fr(const b200_fr* p) { Fr r; memcpy(&r, p, sizeof r); return
 // 24: 9.0 / 6.0 vs 5.8 / 6.1;  28: 10.1 / 8.1 vs 6.3 / 6.2;  32: 21.3 / 20.8 vs 13.0 / 11.9.  The crossover is at about 24 MiB.
 static constexpr size_t BOUNCE_BYTES = (size_t)16 << 20;
 static constexpr size_t DIRECT_MAX_BYTES = (size_t)24 << 20;
-struct HostSeg { uint8_t* p; size_t bytes; };          // one caller buffer (a column); a list of them maps onto ONE contiguous device range
+// One caller buffer (a column); a list of them maps onto ONE contiguous device range.  stride != 0 (uploads only): the segment is the
+// field elements p[0], p[stride], p[2 stride], ... (bytes / 32 of them, stride in bytes), gathered on the host into the pinned slot.
+struct HostSeg { uint8_t* p; size_t bytes; size_t stride = 0; };
 // copies bytes [lo, hi) of the virtual concatenation of `segs` between the caller's buffers and `flat` (the pinned slot, offset 0 = byte lo0)
 static void seg_copy_range(const HostSeg* segs, size_t nsegs, size_t lo0, size_t lo, size_t hi, uint8_t* flat, bool to_flat) {
     size_t pos = 0;
@@ -209,7 +211,10 @@ static void seg_copy_range(const HostSeg* segs, size_t nsegs, size_t lo0, size_t
         pos = s1;
         if (s1 <= lo) continue;
         const size_t a = lo > s0 ? lo : s0, b = hi < s1 ? hi : s1;
-        if (to_flat) memcpy(flat + (a - lo0), segs[i].p + (a - s0), b - a);
+        if (segs[i].stride) {           // chunk and segment edges are multiples of 32 B, so [a, b) holds whole elements
+            for (size_t e = (a - s0) / sizeof(Fr); e < (b - s0) / sizeof(Fr); ++e)
+                memcpy(flat + (s0 + e * sizeof(Fr) - lo0), segs[i].p + e * segs[i].stride, sizeof(Fr));
+        } else if (to_flat) memcpy(flat + (a - lo0), segs[i].p + (a - s0), b - a);
         else memcpy(segs[i].p + (a - s0), flat + (a - lo0), b - a);
     }
 }
@@ -237,8 +242,9 @@ static int bounce_ready(Ctx* c) {
 // caller buffers -> contiguous device range.  When the call returns every SOURCE has been read; the device copies are ordered on `st`.
 static int h2d_segments(Ctx* c, void* d_dst, const HostSeg* segs, size_t nsegs, cudaStream_t st) {
     size_t total = 0;
-    for (size_t i = 0; i < nsegs; ++i) total += segs[i].bytes;
-    if (total < DIRECT_MAX_BYTES) {
+    bool strided = false;
+    for (size_t i = 0; i < nsegs; ++i) { total += segs[i].bytes; strided |= segs[i].stride != 0; }
+    if (total < DIRECT_MAX_BYTES && !strided) {
         size_t off = 0;
         for (size_t i = 0; i < nsegs; ++i) { B200_CUDA(cudaMemcpyAsync((uint8_t*)d_dst + off, segs[i].p, segs[i].bytes, cudaMemcpyHostToDevice, st)); off += segs[i].bytes; }
         return 0;
@@ -1209,7 +1215,7 @@ int b200_lookup_multiplicities(const b200_fr* table, size_t n_table, const b200_
 // ---- quotient numerator (evaluate_h) ------------------------------------------------------------------------------
 static_assert(sizeof(b200_instr) == sizeof(QInstr) && sizeof(b200_col_ref) == sizeof(QLoad), "ABI structs must match the kernel's");
 static int quotient_eval_on(Ctx* c, cudaStream_t st, const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
-                            const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out) {
+                            const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out, uint32_t out_shift = 0, uint32_t out_off = 0) {
     B200_CHECK(d_out && (n_columns == 0 || d_columns) && (n_loads == 0 || loads) && (n_constants == 0 || constants) && (n_instr == 0 || program), -1, "quotient_eval: null pointer");
     B200_CHECK(ext_k >= k && ext_k <= 28, -1, "quotient_eval: need k <= ext_k <= 28");
     const uint64_t N = 1ull << ext_k, scale = 1ull << (ext_k - k);
@@ -1220,7 +1226,7 @@ static int quotient_eval_on(Ctx* c, cudaStream_t st, const void* const* d_column
         ql[i].offset = (uint32_t)(((off % (int64_t)N) + (int64_t)N) % (int64_t)N);
     }
     return quotient_eval_run(reinterpret_cast<const Fr* const*>(d_columns), n_columns, ext_k, ql.data(), n_loads, reinterpret_cast<const Fr*>(constants), n_constants,
-                             reinterpret_cast<const QInstr*>(program), n_instr, reinterpret_cast<Fr*>(d_out), c->ring, st);
+                             reinterpret_cast<const QInstr*>(program), n_instr, reinterpret_cast<Fr*>(d_out), out_shift, out_off, c->ring, st);
 }
 int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
                            const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out, void* stream) {
@@ -1247,30 +1253,19 @@ int b200_quotient_eval(const b200_fr* const* columns, size_t n_columns, uint32_t
     return d2h_one(c, out, c->stage_b.p, sizeof(Fr) * N, ss.st);
 }
 
-// evaluate_h at its natural boundary: the CPU evaluator receives coefficient-form polynomials and builds their cosets itself
-// (UPSTREAM plonk/evaluation.rs: `advice_polys.iter().map(|a| domain.coeff_to_extended(a))`), and vanishing/prover.rs then divides by
-// the vanishing polynomial and converts back.  One call does the same on the device, so a coefficient column crosses PCIe once
-// (n elements) instead of its coset twice (2^ext_k down, 2^ext_k up).
-int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta,
-                    const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr,
-                    const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, b200_fr* out) {
-    B200_ENTER(c, nullptr);
-    B200_CHECK(out && ext_omega && zeta && (n_columns == 0 || (polys && lengths)), -1, "evaluate_h: null pointer");
-    B200_CHECK(ext_k >= k && ext_k >= 1 && ext_k <= 28, -1, "evaluate_h: need k <= ext_k <= 28");
-    B200_CHECK(!t_evaluations || (t_period >= 1 && t_period <= 1024 && ext_omega_inv && ext_ifft_divisor), -1, "evaluate_h: finishing needs t_evaluations, its period and the inverse-transform constants");
+// evaluate_h with every column's extended coset resident: stage_c = the cosets, stage_a = coefficient staging (one sub-batch),
+// stage_b = NTT scratch / output.  On return h = stage_b[0, N) and stage_c is free.
+static int evaluate_h_cosets(Ctx* c, cudaStream_t st, const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
+                             const b200_fr* ext_omega, const b200_fr* zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
+                             const b200_instr* program, size_t n_instr) {
     const size_t N = (size_t)1 << ext_k;
-    size_t n_coeff_cols = 0, max_len = 0;
-    for (size_t i = 0; i < n_columns; ++i) {
-        B200_CHECK(polys[i] && lengths[i] >= 1 && lengths[i] <= N, -1, "evaluate_h: column %zu is null or longer than 2^ext_k", i);
-        if (lengths[i] < N) { ++n_coeff_cols; if (lengths[i] > max_len) max_len = lengths[i]; }
-    }
-    // device layout: stage_c = every column on the extended domain, stage_a = coefficient staging (one sub-batch), stage_b = NTT scratch / output
     if (c->stage_c.ensure(sizeof(Fr) * N * (n_columns ? n_columns : 1))) return -2;
+    size_t n_coeff_cols = 0, max_len = 0;
+    for (size_t i = 0; i < n_columns; ++i) if (lengths[i] < N) { ++n_coeff_cols; if (lengths[i] > max_len) max_len = lengths[i]; }
     size_t sub = n_coeff_cols ? call_budget() / (sizeof(Fr) * (N + max_len)) : 1;
     if (sub < 1) sub = 1;
     if (sub > n_coeff_cols) sub = n_coeff_cols ? n_coeff_cols : 1;
     if (c->stage_a.ensure(sizeof(Fr) * (max_len ? max_len : 1) * sub) || c->stage_b.ensure(sizeof(Fr) * N * sub)) return -2;
-    StreamScope ss(c, nullptr);
     Fr* ext = c->stage_c.as<Fr>();
     NttScale pre, none;
     pre.mode = 3; pre.c[0] = fp_one<FrTag>(); pre.c[1] = as_fr(zeta); pre.c[2] = as_fr(zeta) * as_fr(zeta);
@@ -1279,23 +1274,23 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
         if (group.empty()) return 0;
         std::vector<HostSeg> up(group.size());
         for (size_t p = 0; p < group.size(); ++p) up[p] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[group[p]]), sizeof(Fr) * len};
-        if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), ss.st)) return rc;
+        if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), st)) return rc;
         // transform into scratch-free destinations: each polynomial lands in its own column of `ext` (dst stride = distance between them is
         // irregular, so one launch per run of consecutive column indices)
         size_t p0 = 0;
         while (p0 < group.size()) {
             size_t p1 = p0 + 1;
             while (p1 < group.size() && group[p1] == group[p1 - 1] + 1) ++p1;
-            if (int rc = ntt_call(c, ss.st, c->stage_a.as<Fr>() + p0 * len, len, len, c->stage_b.as<Fr>(), ext + group[p0] * N, N, ext_k, as_fr(ext_omega), pre, none, (int)(p1 - p0))) return rc;
+            if (int rc = ntt_call(c, st, c->stage_a.as<Fr>() + p0 * len, len, len, c->stage_b.as<Fr>(), ext + group[p0] * N, N, ext_k, as_fr(ext_omega), pre, none, (int)(p1 - p0))) return rc;
             p0 = p1;
         }
-        B200_CUDA(cudaStreamSynchronize(ss.st));          // the coefficient staging buffer is reused by the next group
+        B200_CUDA(cudaStreamSynchronize(st));          // the coefficient staging buffer is reused by the next group
         group.clear();
         return 0;
     };
     size_t cur_len = 0;
     for (size_t i = 0; i < n_columns; ++i) {
-        if (lengths[i] == N) { if (int rc = h2d_one(c, ext + i * N, polys[i], sizeof(Fr) * N, ss.st)) return rc; continue; }
+        if (lengths[i] == N) { if (int rc = h2d_one(c, ext + i * N, polys[i], sizeof(Fr) * N, st)) return rc; continue; }
         if (!group.empty() && (lengths[i] != cur_len || group.size() == sub)) { if (int rc = flush(cur_len)) return rc; }
         cur_len = lengths[i];
         group.push_back(i);
@@ -1303,14 +1298,109 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
     if (int rc = flush(cur_len)) return rc;
     std::vector<const void*> ptrs(n_columns);
     for (size_t i = 0; i < n_columns; ++i) ptrs[i] = ext + i * N;
+    return quotient_eval_on(c, st, ptrs.data(), n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, c->stage_b.p);
+}
+
+// evaluate_h by parts: the extended domain of N = d n points is the disjoint union of the d cosets of the n-point domain; part c
+// holds the extended indices c + d i (the points g_c w_n^i, g_c = zeta w_N^c).  A rotation by r rows moves c + d i to
+// c + d ((i + r) mod n), inside part c, so the numerator on part c reads only part c of every column: n elements per column.
+//   coefficient columns: uploaded once, into stage_a; part c of column p is the size-n NTT (w_n = w_N^d) of
+//                        b_s = sum_q p_{s+qn} g_c^{s+qn}, folded and pre-scaled by poly_coset_fold from two small power tables of w_N;
+//   extended columns:    elements c, c + d, ... gathered on the host into the pinned bounce slots, n per column;
+//   numerator:           the interpreter at (k, k), storing row i at index c + d i of h.
+// Device memory: stage_c = n_columns parts (n each), stage_a = the coefficient columns, stage_b = h and an N-element NTT scratch.
+// On return h = stage_b[0, N) and stage_b[N, 2N) is free.
+static int evaluate_h_parts(Ctx* c, cudaStream_t st, const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
+                            const Fr& ext_omega, const Fr& zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
+                            const b200_instr* program, size_t n_instr) {
+    const size_t N = (size_t)1 << ext_k, n = (size_t)1 << k, d = N >> k;
+    // part slots: the coefficient columns in column order, then the extended columns (one contiguous upload per part)
+    std::vector<size_t> coeff, exts;
+    size_t coeff_elems = 0;
+    for (size_t i = 0; i < n_columns; ++i) {
+        if (lengths[i] < N) { coeff.push_back(i); coeff_elems += lengths[i]; }
+        else exts.push_back(i);
+    }
+    const uint32_t lo_bits = (ext_k + 1) / 2;
+    const size_t n_lo = (size_t)1 << lo_bits, n_hi = N >> lo_bits;
+    if (c->stage_c.ensure(sizeof(Fr) * n * n_columns) || c->stage_a.ensure(sizeof(Fr) * (coeff_elems ? coeff_elems : 1)) || c->stage_b.ensure(sizeof(Fr) * 2 * N) ||
+        c->small.ensure(sizeof(Fr) * (3 + n_lo + n_hi))) return -2;
+    Fr* parts = c->stage_c.as<Fr>();
     Fr* h = c->stage_b.as<Fr>();
-    if (int rc = quotient_eval_on(c, ss.st, ptrs.data(), n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, h)) return rc;
+    Fr* tmp = h + N;
+    // [1, zeta, zeta^2 | w_N^e, e < n_lo | w_N^(e n_lo), e < n_hi]
+    std::vector<Fr> tab(3 + n_lo + n_hi);
+    tab[0] = fp_one<FrTag>(); tab[1] = zeta; tab[2] = zeta * zeta;
+    Fr* lo = tab.data() + 3;
+    Fr* hi = lo + n_lo;
+    lo[0] = fp_one<FrTag>();
+    for (size_t e = 1; e < n_lo; ++e) lo[e] = lo[e - 1] * ext_omega;
+    const Fr step = lo[n_lo - 1] * ext_omega;
+    hi[0] = fp_one<FrTag>();
+    for (size_t e = 1; e < n_hi; ++e) hi[e] = hi[e - 1] * step;
+    if (int rc = h2d_one(c, c->small.p, tab.data(), sizeof(Fr) * tab.size(), st)) return rc;
+    Fr omega_n = ext_omega;
+    for (uint32_t i = k; i < ext_k; ++i) omega_n = omega_n * omega_n;
+    std::vector<HostSeg> up(coeff.size()), ext_up(exts.size());
+    for (size_t j = 0; j < coeff.size(); ++j) up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[coeff[j]]), sizeof(Fr) * lengths[coeff[j]]};
+    if (!coeff.empty()) { if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), st)) return rc; }
+    std::vector<const void*> ptrs(n_columns);
+    for (size_t j = 0; j < coeff.size(); ++j) ptrs[coeff[j]] = parts + j * n;
+    for (size_t j = 0; j < exts.size(); ++j) ptrs[exts[j]] = parts + (coeff.size() + j) * n;
+    NttScale none;
+    for (size_t part = 0; part < d; ++part) {
+        // coefficient columns: runs of equal length, at most d per transform (the scratch holds d parts)
+        size_t off = 0;
+        for (size_t j0 = 0; j0 < coeff.size();) {
+            const size_t len = lengths[coeff[j0]];
+            size_t j1 = j0 + 1;
+            while (j1 < coeff.size() && j1 - j0 < d && lengths[coeff[j1]] == len) ++j1;
+            const int nb = (int)(j1 - j0);
+            if (int rc = poly_coset_fold(c->stage_a.as<Fr>() + off, len, len, c->small.as<Fr>(), lo_bits, ext_k, part, parts + j0 * n, n, n, nb, st)) return rc;
+            if (int rc = ntt_call(c, st, parts + j0 * n, n, n, tmp, parts + j0 * n, n, k, omega_n, none, none, nb)) return rc;
+            off += len * nb;
+            j0 = j1;
+        }
+        for (size_t j = 0; j < exts.size(); ++j) ext_up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[exts[j]] + part), sizeof(Fr) * n, d > 1 ? sizeof(Fr) * d : 0};
+        if (!exts.empty()) { if (int rc = h2d_segments(c, parts + coeff.size() * n, ext_up.data(), ext_up.size(), st)) return rc; }
+        if (int rc = quotient_eval_on(c, st, ptrs.data(), n_columns, k, k, loads, n_loads, constants, n_constants, program, n_instr, h, ext_k - k, (uint32_t)part)) return rc;
+    }
+    return 0;
+}
+
+// evaluate_h at its natural boundary: the CPU evaluator receives coefficient-form polynomials and builds their cosets itself
+// (UPSTREAM plonk/evaluation.rs: `advice_polys.iter().map(|a| domain.coeff_to_extended(a))`), and vanishing/prover.rs then divides by
+// the vanishing polynomial and converts back.  One call does the same on the device, so a coefficient column crosses PCIe once
+// (n elements) instead of its coset twice (2^ext_k down, 2^ext_k up).  When every column's extended coset fits the call budget they
+// are all resident at once; otherwise the numerator is evaluated one n-point coset part at a time (evaluate_h_parts).
+int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta,
+                    const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr,
+                    const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, b200_fr* out) {
+    B200_ENTER(c, nullptr);
+    B200_CHECK(out && ext_omega && zeta && (n_columns == 0 || (polys && lengths)), -1, "evaluate_h: null pointer");
+    B200_CHECK(ext_k >= k && ext_k >= 1 && ext_k <= 28, -1, "evaluate_h: need k <= ext_k <= 28");
+    B200_CHECK(!t_evaluations || (t_period >= 1 && t_period <= 1024 && ext_omega_inv && ext_ifft_divisor), -1, "evaluate_h: finishing needs t_evaluations, its period and the inverse-transform constants");
+    const size_t N = (size_t)1 << ext_k;
+    for (size_t i = 0; i < n_columns; ++i)
+        B200_CHECK(polys[i] && lengths[i] >= 1 && lengths[i] <= N, -1, "evaluate_h: column %zu is null or longer than 2^ext_k", i);
+    StreamScope ss(c, nullptr);
+    Fr* h = nullptr;
+    Fr* scratch = nullptr;
+    if (k >= 1 && sizeof(Fr) * N * n_columns > call_budget()) {
+        if (int rc = evaluate_h_parts(c, ss.st, polys, lengths, n_columns, k, ext_k, as_fr(ext_omega), as_fr(zeta), loads, n_loads, constants, n_constants, program, n_instr)) return rc;
+        h = c->stage_b.as<Fr>();
+        scratch = h + N;
+    } else {
+        if (int rc = evaluate_h_cosets(c, ss.st, polys, lengths, n_columns, k, ext_k, ext_omega, zeta, loads, n_loads, constants, n_constants, program, n_instr)) return rc;
+        h = c->stage_b.as<Fr>();
+        scratch = c->stage_c.as<Fr>();
+    }
     if (t_evaluations) {
         if (int rc = scale_cycle_on(c, ss.st, h, N, t_evaluations, t_period)) return rc;
-        NttScale post;
         const Fr z = as_fr(zeta), z2 = z * z, d = as_fr(ext_ifft_divisor);
+        NttScale none, post;
         post.mode = 3; post.c[0] = d; post.c[1] = d * z2; post.c[2] = d * z;
-        if (int rc = ntt_call(c, ss.st, h, N, N, ext, h, N, ext_k, as_fr(ext_omega_inv), none, post, 1)) return rc;      // `ext` is free again: scratch
+        if (int rc = ntt_call(c, ss.st, h, N, N, scratch, h, N, ext_k, as_fr(ext_omega_inv), none, post, 1)) return rc;
     }
     return d2h_one(c, out, h, sizeof(Fr) * N, ss.st);
 }

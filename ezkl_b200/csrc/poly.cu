@@ -74,6 +74,34 @@ int poly_scale_cycle(const Fr* a, const Fr* h_consts, uint32_t period, Fr* out, 
     return 0;
 }
 
+// column blockIdx.y: out[s] = sum_{t = s + q n < len} a[t] * cyc[t mod 3] * w^(mul * t mod 2^log_w), s < n.  tab = [cyc[3] | lo | hi] with
+// w^e = lo[e mod 2^lo_bits] * hi[e >> lo_bits].
+__global__ void __launch_bounds__(256) k_poly_coset_fold(const Fr* __restrict__ a_all, size_t a_stride, size_t len, const Fr* __restrict__ tab, uint32_t lo_bits,
+                                                         uint64_t mul, uint64_t emask, Fr* __restrict__ out_all, size_t out_stride, size_t n) {
+    const Fr* a = a_all + (size_t)blockIdx.y * a_stride;
+    Fr* out = out_all + (size_t)blockIdx.y * out_stride;
+    const Fr* lo = tab + 3;
+    const Fr* hi = lo + ((size_t)1 << lo_bits);
+    const uint64_t lo_mask = ((uint64_t)1 << lo_bits) - 1;
+    for (size_t s = (size_t)blockIdx.x * blockDim.x + threadIdx.x; s < n; s += (size_t)gridDim.x * blockDim.x) {
+        Fr acc = fp_zero<FrTag>();
+#pragma unroll 1
+        for (size_t t = s; t < len; t += n) {
+            const uint64_t e = (mul * t) & emask;
+            acc = acc + fp_load(a + t) * (fp_load(tab + t % 3) * (fp_load(lo + (e & lo_mask)) * fp_load(hi + (e >> lo_bits))));
+        }
+        fp_store(out + s, acc);
+    }
+}
+int poly_coset_fold(const Fr* a, size_t a_stride, size_t len, const Fr* d_tab, uint32_t lo_bits, uint32_t log_w, uint64_t mul, Fr* out, size_t out_stride, size_t n,
+                    int batch, cudaStream_t st) {
+    B200_CHECK(batch > 0 && batch <= 65535 && n > 0 && lo_bits <= log_w && log_w <= 28, -1, "poly_coset_fold: bad argument");
+    k_poly_coset_fold<<<dim3(ew_grid(n), batch), 256, 0, st>>>(a, a_stride, len, d_tab, lo_bits, mul, ((uint64_t)1 << log_w) - 1, out, out_stride, n);
+    count_launch();
+    B200_CUDA(cudaGetLastError());
+    return 0;
+}
+
 // ---- shared-memory helpers for one Fr per thread -------------------------------------------------------------
 DEV Fr shf_get(const Fr* sh, uint32_t i) { return fp_load(sh + i); }
 DEV void shf_put(Fr* sh, uint32_t i, const Fr& v) { fp_store(sh + i, v); }

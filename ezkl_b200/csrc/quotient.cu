@@ -20,7 +20,7 @@ struct QLoadDev { const Fr* col; uint32_t offset, pad; };      // 16 B: column p
 
 template <int NSLOT>
 __global__ void __launch_bounds__(128) k_quotient_eval(const uint4* __restrict__ blob, uint32_t blob_u4, uint32_t o_loads_u4, uint32_t o_consts_u4, uint32_t mask,
-                                                        uint32_t n_instr, Fr* __restrict__ out) {
+                                                        uint32_t n_instr, Fr* __restrict__ out, uint32_t out_shift, uint32_t out_off) {
     extern __shared__ uint4 sh[];
     for (uint32_t i = threadIdx.x; i < blob_u4; i += blockDim.x) sh[i] = blob[i];
     __syncthreads();
@@ -58,12 +58,13 @@ __global__ void __launch_bounds__(128) k_quotient_eval(const uint4* __restrict__
         if (!(in.op_dst & Q_NOSTORE)) slots[(in.op_dst >> 8) & (NSLOT - 1)] = r;
         prev = r;
     }
-    fp_store(out + idx, prev);           // the row's result is the last instruction's (zero for an empty program)
+    fp_store(out + ((idx << out_shift) + out_off), prev);      // the row's result is the last instruction's (zero for an empty program)
 }
 
 int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k, const QLoad* h_loads, size_t n_loads, const Fr* h_consts, size_t n_consts,
-                      const QInstr* h_prog, size_t n_instr, Fr* d_out, StagingRing& ring, cudaStream_t st) {
+                      const QInstr* h_prog, size_t n_instr, Fr* d_out, uint32_t out_shift, uint32_t out_off, StagingRing& ring, cudaStream_t st) {
     B200_CHECK(ext_k >= 1 && ext_k <= 28, -1, "quotient_eval: ext_k %u out of range", ext_k);
+    B200_CHECK(ext_k + out_shift <= 28 && out_off < (1u << out_shift), -1, "quotient_eval: output layout out of range");
     B200_CHECK(n_instr < (1u << 24) && n_loads < (1u << 30) && n_consts < (1u << 30), -1, "quotient_eval: program too large");
     const uint32_t N = 1u << ext_k;
     // validate the program on the host so the kernel can index without checks
@@ -102,7 +103,7 @@ int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k
     do {                                                                                                                              \
         B200_CUDA(cudaFuncSetAttribute(k_quotient_eval<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024 + 64));            \
         k_quotient_eval<NS><<<grid, 128, smem, st>>>(reinterpret_cast<const uint4*>(d), blob_u4, (uint32_t)(o_loads / 16), (uint32_t)(o_consts / 16), N - 1, \
-                                                     (uint32_t)n_instr, d_out);                                                        \
+                                                     (uint32_t)n_instr, d_out, out_shift, out_off);                                    \
     } while (0)
     if (max_slot < 32) B200_QLAUNCH(32);
     else if (max_slot < 64) B200_QLAUNCH(64);

@@ -291,7 +291,8 @@ def evaluate_h(program: QuotientProgram, columns, k: int, ext_k: int) -> np.ndar
 def evaluate_h_from_polys(program: QuotientProgram, polys, domain, finish: bool = False) -> np.ndarray:
     """b200_evaluate_h: columns given as the prover holds them — coefficient form (len < 2^ext_k: the library builds the coset) or already on
     the extended domain (len == 2^ext_k).  `domain` is a halo2.EvaluationDomain; finish=True also divides by the vanishing polynomial
-    and returns the quotient's coefficients (all 2^ext_k of them)."""
+    and returns the quotient's coefficients (all 2^ext_k of them).  When the columns' extended cosets exceed the library's per-call
+    budget the numerator is evaluated one n-point coset part at a time (include/ezkl_b200.h), with the same result."""
     nat.ensure_init()
     cols = [nat.as_u64(c, 4) for c in polys]
     N = 1 << domain.extended_k

@@ -206,8 +206,12 @@ int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint3
  * program is coeff_to_extended(polys[i]) when lengths[i] < 2^ext_k (coefficient form, zeta coset, zero padded) and polys[i] itself when
  * lengths[i] == 2^ext_k (the key's fixed / permutation cosets, l0 / l_last / l_active_row, a running partial sum).  out = the numerator on
  * the extended domain, or, when t_evaluations != NULL, extended_to_coeff(numerator * t_evaluations[i mod t_period]): the quotient's
- * 2^ext_k coefficients.  A coefficient column crosses PCIe once (its n elements) instead of its coset twice.  All columns' cosets are
- * resident during the call (n_columns * 2^ext_k * 32 B): split larger systems into partial sums carried as an extended column. */
+ * 2^ext_k coefficients.  A coefficient column crosses PCIe once (its n elements) instead of its coset twice.
+ * Device memory: when n_columns * 2^ext_k * 32 B fits the per-call scratch budget (B200_WS_BUDGET_MB, else derived from
+ * B200_WS_TOTAL_MB, as for every host-pointer entry point) all columns' cosets are resident at once.  Otherwise (and k >= 1) the
+ * numerator is evaluated one n-point coset part at a time (the extended indices c + d i, d = 2^(ext_k - k), for c < d), which holds
+ * about n_columns * n * 32 B + (sum of the coefficient columns' lengths) * 32 B + 2 * 2^ext_k * 32 B.  The result is the same bytes
+ * either way. */
 int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta,
                     const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr,
                     const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, b200_fr* out);

@@ -15,6 +15,38 @@ from ezkl_b200 import device as dev  # noqa: E402
 from ezkl_b200 import evaluation as ev  # noqa: E402
 
 
+def ezkl_system(blocks):
+    """(program, number of columns, the columns a prover holds in coefficient form: advice, z, m, phi)."""
+    col = 0
+
+    def new(cnt):
+        nonlocal col
+        r = list(range(col, col + cnt))
+        col += cnt
+        return r
+
+    terms, perm_cols, coeff = [], [], []
+    blks = []
+    for _ in range(blocks):
+        adv, sel = new(5), new(5)
+        blks.append((adv, sel))
+        coeff += adv
+        terms += ev.base_op_gates(dict(zip(["ADD", "MULT", "DOTINIT", "DOT", "SUM"], sel)), adv[0:2], adv[2:4], adv[4])
+        perm_cols += [adv[0], adv[2], adv[4]]
+    sig = new(len(perm_cols))
+    nz = (len(perm_cols) + 2) // 3
+    zs = new(nz)
+    coeff += zs
+    l0, l_last, l_active, xcol = new(4)
+    terms += ev.permutation_terms(perm_cols, sig, zs, l0, l_last, l_active, xcol, 11, 13, 3, 5)
+    for b in range(0, blocks, 2):
+        table, sel_l, m, phi = new(4)
+        coeff += [m, phi]
+        f = ev.Query(sel_l) * ev.Query(blks[b][0][1]) + (ev.Constant(1) - ev.Query(sel_l)) * ev.Constant(7)
+        terms += ev.mv_lookup_terms([f], ev.Query(table), m, phi, l0, l_last, l_active, 17)
+    return ev.QuotientProgram(ev.fold_y(terms, 99)), col, set(coeff)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--blocks", type=int, default=8)
@@ -25,35 +57,10 @@ def main():
     nat.init(0)
     k, ext_k = a.k, a.k + a.ext_bits
     N = 1 << ext_k
-    col = 0
-
-    def new(cnt):
-        nonlocal col
-        r = list(range(col, col + cnt))
-        col += cnt
-        return r
-
-    terms, perm_cols = [], []
-    blocks = []
-    for _ in range(a.blocks):
-        adv, sel = new(5), new(5)
-        blocks.append((adv, sel))
-        terms += ev.base_op_gates(dict(zip(["ADD", "MULT", "DOTINIT", "DOT", "SUM"], sel)), adv[0:2], adv[2:4], adv[4])
-        perm_cols += [adv[0], adv[2], adv[4]]
-    sig = new(len(perm_cols))
-    nz = (len(perm_cols) + 2) // 3
-    zs = new(nz)
-    l0, l_last, l_active, xcol = new(4)
-    terms += ev.permutation_terms(perm_cols, sig, zs, l0, l_last, l_active, xcol, 11, 13, 3, 5)
-    for b in range(0, a.blocks, 2):
-        table, sel_l, m, phi = new(4)
-        f = ev.Query(sel_l) * ev.Query(blocks[b][0][1]) + (ev.Constant(1) - ev.Query(sel_l)) * ev.Constant(7)
-        terms += ev.mv_lookup_terms([f], ev.Query(table), m, phi, l0, l_last, l_active, 17)
-    prog = ev.QuotientProgram(ev.fold_y(terms, 99))
-    ncols = col
+    prog, ncols, _ = ezkl_system(a.blocks)
     distinct = len(prog.loads)
-    print("columns %d, terms %d, instructions %d (muladd %d), slots %d, distinct (column, rotation) loads %d, constants %d" %
-          (ncols, len(terms), len(prog.instrs), sum(1 for i in prog.instrs if i[0] == ev.OP_MULADD), prog.n_slots, distinct, len(prog.consts)), flush=True)
+    print("columns %d, instructions %d (muladd %d), slots %d, distinct (column, rotation) loads %d, constants %d" %
+          (ncols, len(prog.instrs), sum(1 for i in prog.instrs if i[0] == ev.OP_MULADD), prog.n_slots, distinct, len(prog.consts)), flush=True)
     pool = dev.random_scalars(N, batch=ncols, seed=3)                        # every column its own buffer (132 x 32 MB at the defaults)
     columns = [pool[i % pool.shape[0]] for i in range(ncols)]
     out = torch.empty((N, 4), dtype=torch.int64, device="cuda")
