@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "../../include/ezkl_b200.h"
+#include "../../include/ezkl_b200_resident.h"
 #include "msm.cuh"
 #include "ntt.cuh"
 #include "poly.cuh"
@@ -283,6 +284,17 @@ static int d2h_segments(Ctx* c, const void* d_src, const HostSeg* segs, size_t n
             B200_CUDA(cudaEventSynchronize(c->bounce_ev[(i - 1) & 1]));
             seg_copy_parallel(segs, nsegs, off, off + nb, c->bounce[(i - 1) & 1], false);
         }
+    }
+    return 0;
+}
+// small host parameter tables -> a device buffer of the context, through the staging ring in slot-sized pieces (pinned, asynchronous, ordered
+// on `st`); unlike a ring slot, the destination stays valid for as many later launches as the call makes
+static int ring_upload(Ctx* c, void* d_dst, const void* h_src, size_t bytes, cudaStream_t st) {
+    for (size_t off = 0; off < bytes; off += StagingRing::SLOT) {
+        const size_t nb = bytes - off < StagingRing::SLOT ? bytes - off : StagingRing::SLOT;
+        const void* d;
+        if (int rc = c->ring.push((const uint8_t*)h_src + off, nb, st, &d)) return rc;
+        B200_CUDA(cudaMemcpyAsync((uint8_t*)d_dst + off, d, nb, cudaMemcpyDeviceToDevice, st));
     }
     return 0;
 }
@@ -1215,7 +1227,8 @@ int b200_lookup_multiplicities(const b200_fr* table, size_t n_table, const b200_
 // ---- quotient numerator (evaluate_h) ------------------------------------------------------------------------------
 static_assert(sizeof(b200_instr) == sizeof(QInstr) && sizeof(b200_col_ref) == sizeof(QLoad), "ABI structs must match the kernel's");
 static int quotient_eval_on(Ctx* c, cudaStream_t st, const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
-                            const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out, uint32_t out_shift = 0, uint32_t out_off = 0) {
+                            const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr, void* d_out, uint32_t out_shift = 0, uint32_t out_off = 0,
+                            const uint32_t* col_shifts = nullptr) {
     B200_CHECK(d_out && (n_columns == 0 || d_columns) && (n_loads == 0 || loads) && (n_constants == 0 || constants) && (n_instr == 0 || program), -1, "quotient_eval: null pointer");
     B200_CHECK(ext_k >= k && ext_k <= 28, -1, "quotient_eval: need k <= ext_k <= 28");
     const uint64_t N = 1ull << ext_k, scale = 1ull << (ext_k - k);
@@ -1225,7 +1238,7 @@ static int quotient_eval_on(Ctx* c, cudaStream_t st, const void* const* d_column
         const int64_t off = (int64_t)loads[i].rotation * (int64_t)scale;           // Rotation(r) on the extended domain = r * 2^(ext_k - k)
         ql[i].offset = (uint32_t)(((off % (int64_t)N) + (int64_t)N) % (int64_t)N);
     }
-    return quotient_eval_run(reinterpret_cast<const Fr* const*>(d_columns), n_columns, ext_k, ql.data(), n_loads, reinterpret_cast<const Fr*>(constants), n_constants,
+    return quotient_eval_run(reinterpret_cast<const Fr* const*>(d_columns), col_shifts, n_columns, ext_k, ql.data(), n_loads, reinterpret_cast<const Fr*>(constants), n_constants,
                              reinterpret_cast<const QInstr*>(program), n_instr, reinterpret_cast<Fr*>(d_out), out_shift, out_off, c->ring, st);
 }
 int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
@@ -1303,69 +1316,108 @@ static int evaluate_h_cosets(Ctx* c, cudaStream_t st, const b200_fr* const* poly
 
 // evaluate_h by parts: the extended domain of N = d n points is the disjoint union of the d cosets of the n-point domain; part c
 // holds the extended indices c + d i (the points g_c w_n^i, g_c = zeta w_N^c).  A rotation by r rows moves c + d i to
-// c + d ((i + r) mod n), inside part c, so the numerator on part c reads only part c of every column: n elements per column.
-//   coefficient columns: uploaded once, into stage_a; part c of column p is the size-n NTT (w_n = w_N^d) of
-//                        b_s = sum_q p_{s+qn} g_c^{s+qn}, folded and pre-scaled by poly_coset_fold from two small power tables of w_N;
-//   extended columns:    elements c, c + d, ... gathered on the host into the pinned bounce slots, n per column;
+// c + d ((i + r) mod n), inside part c, so the numerator on part c reads only part c of every column: n elements per column.  Per part:
+//   coefficient columns: part c of column p is the size-n NTT (w_n = w_N^d) of b_s = sum_q p_{s+qn} g_c^{s+qn}, folded and pre-scaled
+//                        by ONE poly_coset_fold launch for every coefficient column (a device table of (address, length) per column) from
+//                        two small power tables of w_N, then transformed in batches of at most d columns (tmp holds d parts);
+//   extended columns:    read in place by the interpreter, elements c, c + d, c + 2d, ... of cols[i] (a load of stride d from cols[i] + c);
+//                        or, when stage_ext is given, staged by stage_ext(c) as n contiguous elements at cols[i] and read densely;
 //   numerator:           the interpreter at (k, k), storing row i at index c + d i of h.
-// Device memory: stage_c = n_columns parts (n each), stage_a = the coefficient columns, stage_b = h and an N-element NTT scratch.
-// On return h = stage_b[0, N) and stage_b[N, 2N) is free.
-static int evaluate_h_parts(Ctx* c, cudaStream_t st, const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
-                            const Fr& ext_omega, const Fr& zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
-                            const b200_instr* program, size_t n_instr) {
+// cols[i] = device address of column i, lengths[i] < N: coefficient form, == N: extended.  Device memory: parts = n_coeff * n elements (the
+// coefficient columns' parts, in column order), tmp = N elements, and the power and fold tables in c->small.  Both evaluate_h entry points
+// run this loop: the host one on columns it uploads, the _dev one on the caller's.
+static int evaluate_h_parts_on(Ctx* c, cudaStream_t st, const Fr* const* cols, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
+                               const Fr& ext_omega, const Fr& zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
+                               const b200_instr* program, size_t n_instr, Fr* parts, Fr* tmp, Fr* h, const std::function<int(size_t)>& stage_ext) {
     const size_t N = (size_t)1 << ext_k, n = (size_t)1 << k, d = N >> k;
-    // part slots: the coefficient columns in column order, then the extended columns (one contiguous upload per part)
-    std::vector<size_t> coeff, exts;
-    size_t coeff_elems = 0;
-    for (size_t i = 0; i < n_columns; ++i) {
-        if (lengths[i] < N) { coeff.push_back(i); coeff_elems += lengths[i]; }
-        else exts.push_back(i);
-    }
+    std::vector<FoldCol> fold;
+    for (size_t i = 0; i < n_columns; ++i) if (lengths[i] < N) fold.push_back(FoldCol{cols[i], lengths[i]});
     const uint32_t lo_bits = (ext_k + 1) / 2;
-    const size_t n_lo = (size_t)1 << lo_bits, n_hi = N >> lo_bits;
-    if (c->stage_c.ensure(sizeof(Fr) * n * n_columns) || c->stage_a.ensure(sizeof(Fr) * (coeff_elems ? coeff_elems : 1)) || c->stage_b.ensure(sizeof(Fr) * 2 * N) ||
-        c->small.ensure(sizeof(Fr) * (3 + n_lo + n_hi))) return -2;
-    Fr* parts = c->stage_c.as<Fr>();
-    Fr* h = c->stage_b.as<Fr>();
-    Fr* tmp = h + N;
-    // [1, zeta, zeta^2 | w_N^e, e < n_lo | w_N^(e n_lo), e < n_hi]
-    std::vector<Fr> tab(3 + n_lo + n_hi);
+    const size_t n_lo = (size_t)1 << lo_bits, n_hi = N >> lo_bits, n_tab = 3 + n_lo + n_hi;
+    // [1, zeta, zeta^2 | w_N^e, e < n_lo | w_N^(e n_lo), e < n_hi | the fold table], staged once for every part
+    const size_t tab_bytes = sizeof(Fr) * n_tab, fold_bytes = sizeof(FoldCol) * fold.size();
+    if (c->small.ensure(tab_bytes + fold_bytes)) return -2;
+    std::vector<uint8_t> blob(tab_bytes + fold_bytes);
+    Fr* tab = reinterpret_cast<Fr*>(blob.data());
     tab[0] = fp_one<FrTag>(); tab[1] = zeta; tab[2] = zeta * zeta;
-    Fr* lo = tab.data() + 3;
+    Fr* lo = tab + 3;
     Fr* hi = lo + n_lo;
     lo[0] = fp_one<FrTag>();
     for (size_t e = 1; e < n_lo; ++e) lo[e] = lo[e - 1] * ext_omega;
     const Fr step = lo[n_lo - 1] * ext_omega;
     hi[0] = fp_one<FrTag>();
     for (size_t e = 1; e < n_hi; ++e) hi[e] = hi[e - 1] * step;
-    if (int rc = h2d_one(c, c->small.p, tab.data(), sizeof(Fr) * tab.size(), st)) return rc;
+    if (fold_bytes) memcpy(blob.data() + tab_bytes, fold.data(), fold_bytes);
+    if (int rc = ring_upload(c, c->small.p, blob.data(), blob.size(), st)) return rc;
+    const Fr* d_tab = c->small.as<Fr>();
+    const FoldCol* d_fold = reinterpret_cast<const FoldCol*>(c->small.as<uint8_t>() + tab_bytes);
     Fr omega_n = ext_omega;
     for (uint32_t i = k; i < ext_k; ++i) omega_n = omega_n * omega_n;
-    std::vector<HostSeg> up(coeff.size()), ext_up(exts.size());
-    for (size_t j = 0; j < coeff.size(); ++j) up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[coeff[j]]), sizeof(Fr) * lengths[coeff[j]]};
-    if (!coeff.empty()) { if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), st)) return rc; }
     std::vector<const void*> ptrs(n_columns);
-    for (size_t j = 0; j < coeff.size(); ++j) ptrs[coeff[j]] = parts + j * n;
-    for (size_t j = 0; j < exts.size(); ++j) ptrs[exts[j]] = parts + (coeff.size() + j) * n;
+    std::vector<uint32_t> shifts(n_columns, 0);
+    for (size_t i = 0, j = 0; i < n_columns; ++i) if (lengths[i] < N) ptrs[i] = parts + n * j++;
     NttScale none;
     for (size_t part = 0; part < d; ++part) {
-        // coefficient columns: runs of equal length, at most d per transform (the scratch holds d parts)
-        size_t off = 0;
-        for (size_t j0 = 0; j0 < coeff.size();) {
-            const size_t len = lengths[coeff[j0]];
-            size_t j1 = j0 + 1;
-            while (j1 < coeff.size() && j1 - j0 < d && lengths[coeff[j1]] == len) ++j1;
-            const int nb = (int)(j1 - j0);
-            if (int rc = poly_coset_fold(c->stage_a.as<Fr>() + off, len, len, c->small.as<Fr>(), lo_bits, ext_k, part, parts + j0 * n, n, n, nb, st)) return rc;
-            if (int rc = ntt_call(c, st, parts + j0 * n, n, n, tmp, parts + j0 * n, n, k, omega_n, none, none, nb)) return rc;
-            off += len * nb;
-            j0 = j1;
+        if (!fold.empty()) {
+            if (int rc = poly_coset_fold(d_fold, fold.size(), d_tab, lo_bits, ext_k, part, parts, n, n, st)) return rc;
+            for (size_t j0 = 0; j0 < fold.size(); j0 += d) {
+                const int nb = (int)(fold.size() - j0 < d ? fold.size() - j0 : d);
+                if (int rc = ntt_call(c, st, parts + j0 * n, n, n, tmp, parts + j0 * n, n, k, omega_n, none, none, nb)) return rc;
+            }
         }
-        for (size_t j = 0; j < exts.size(); ++j) ext_up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[exts[j]] + part), sizeof(Fr) * n, d > 1 ? sizeof(Fr) * d : 0};
-        if (!exts.empty()) { if (int rc = h2d_segments(c, parts + coeff.size() * n, ext_up.data(), ext_up.size(), st)) return rc; }
-        if (int rc = quotient_eval_on(c, st, ptrs.data(), n_columns, k, k, loads, n_loads, constants, n_constants, program, n_instr, h, ext_k - k, (uint32_t)part)) return rc;
+        if (stage_ext) { if (int rc = stage_ext(part)) return rc; }
+        for (size_t i = 0; i < n_columns; ++i) if (lengths[i] == N) {
+            ptrs[i] = stage_ext ? cols[i] : cols[i] + part;
+            shifts[i] = stage_ext ? 0 : ext_k - k;
+        }
+        if (int rc = quotient_eval_on(c, st, ptrs.data(), n_columns, k, k, loads, n_loads, constants, n_constants, program, n_instr, h, ext_k - k, (uint32_t)part,
+                                      shifts.data())) return rc;
     }
     return 0;
+}
+// the host entry point's parts path: stage_a = the coefficient columns (uploaded once), stage_c = n-element parts of every column (the
+// coefficient columns' in column order, then the extended columns', gathered on the host into the pinned bounce slots per part),
+// stage_b = h and an N-element NTT scratch.  On return h = stage_b[0, N) and stage_b[N, 2N) is free.
+static int evaluate_h_parts(Ctx* c, cudaStream_t st, const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
+                            const Fr& ext_omega, const Fr& zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
+                            const b200_instr* program, size_t n_instr) {
+    const size_t N = (size_t)1 << ext_k, n = (size_t)1 << k, d = N >> k;
+    std::vector<size_t> coeff, exts;
+    size_t coeff_elems = 0;
+    for (size_t i = 0; i < n_columns; ++i) {
+        if (lengths[i] < N) { coeff.push_back(i); coeff_elems += lengths[i]; }
+        else exts.push_back(i);
+    }
+    if (c->stage_c.ensure(sizeof(Fr) * n * n_columns) || c->stage_a.ensure(sizeof(Fr) * (coeff_elems ? coeff_elems : 1)) || c->stage_b.ensure(sizeof(Fr) * 2 * N)) return -2;
+    Fr* parts = c->stage_c.as<Fr>();
+    Fr* h = c->stage_b.as<Fr>();
+    std::vector<HostSeg> up(coeff.size()), ext_up(exts.size());
+    std::vector<const Fr*> cols(n_columns);
+    size_t off = 0;
+    for (size_t j = 0; j < coeff.size(); ++j) {
+        up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[coeff[j]]), sizeof(Fr) * lengths[coeff[j]]};
+        cols[coeff[j]] = c->stage_a.as<Fr>() + off;
+        off += lengths[coeff[j]];
+    }
+    for (size_t j = 0; j < exts.size(); ++j) cols[exts[j]] = parts + (coeff.size() + j) * n;
+    if (!coeff.empty()) { if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), st)) return rc; }
+    auto stage_ext = [&](size_t part) -> int {
+        if (exts.empty()) return 0;
+        for (size_t j = 0; j < exts.size(); ++j) ext_up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[exts[j]] + part), sizeof(Fr) * n, d > 1 ? sizeof(Fr) * d : 0};
+        return h2d_segments(c, parts + coeff.size() * n, ext_up.data(), ext_up.size(), st);
+    };
+    return evaluate_h_parts_on(c, st, cols.data(), lengths, n_columns, k, ext_k, ext_omega, zeta, loads, n_loads, constants, n_constants, program, n_instr,
+                               parts, h + N, h, stage_ext);
+}
+// the finishing step of both evaluate_h entry points, in place in h: h * t_evaluations[i mod t_period], then extended_to_coeff (scratch: N elements)
+static int evaluate_h_finish(Ctx* c, cudaStream_t st, Fr* h, Fr* scratch, uint32_t ext_k, const b200_fr* zeta, const b200_fr* t_evaluations, uint32_t t_period,
+                             const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor) {
+    const size_t N = (size_t)1 << ext_k;
+    if (int rc = scale_cycle_on(c, st, h, N, t_evaluations, t_period)) return rc;
+    const Fr z = as_fr(zeta), z2 = z * z, d = as_fr(ext_ifft_divisor);
+    NttScale none, post;
+    post.mode = 3; post.c[0] = d; post.c[1] = d * z2; post.c[2] = d * z;
+    return ntt_call(c, st, h, N, N, scratch, h, N, ext_k, as_fr(ext_omega_inv), none, post, 1);
 }
 
 // evaluate_h at its natural boundary: the CPU evaluator receives coefficient-form polynomials and builds their cosets itself
@@ -1396,13 +1448,36 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
         scratch = c->stage_c.as<Fr>();
     }
     if (t_evaluations) {
-        if (int rc = scale_cycle_on(c, ss.st, h, N, t_evaluations, t_period)) return rc;
-        const Fr z = as_fr(zeta), z2 = z * z, d = as_fr(ext_ifft_divisor);
-        NttScale none, post;
-        post.mode = 3; post.c[0] = d; post.c[1] = d * z2; post.c[2] = d * z;
-        if (int rc = ntt_call(c, ss.st, h, N, N, scratch, h, N, ext_k, as_fr(ext_omega_inv), none, post, 1)) return rc;
+        if (int rc = evaluate_h_finish(c, ss.st, h, scratch, ext_k, zeta, t_evaluations, t_period, ext_omega_inv, ext_ifft_divisor)) return rc;
     }
     return d2h_one(c, out, h, sizeof(Fr) * N, ss.st);
+}
+
+// evaluate_h on device-resident columns (include/ezkl_b200_resident.h): always by parts, on the caller's columns where they are
+int b200_evaluate_h_dev(const void* const* d_polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta,
+                        const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr,
+                        const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, void* d_out, void* stream) {
+    B200_ENTER(c, d_out);
+    B200_CHECK(d_out && ext_omega && zeta && (n_columns == 0 || (d_polys && lengths)), -1, "evaluate_h_dev: null pointer");
+    B200_CHECK(k >= 1 && ext_k >= k && ext_k <= 28, -1, "evaluate_h_dev: need 1 <= k <= ext_k <= 28 (k = %u, ext_k = %u)", k, ext_k);
+    B200_CHECK(!t_evaluations || (t_period >= 1 && t_period <= 1024 && ext_omega_inv && ext_ifft_divisor), -1,
+               "evaluate_h_dev: finishing needs t_evaluations, a period in 1 ... 1024 and the inverse-transform constants");
+    const size_t N = (size_t)1 << ext_k, n = (size_t)1 << k;
+    const uintptr_t out_lo = (uintptr_t)d_out, out_hi = out_lo + sizeof(Fr) * N;
+    size_t n_coeff = 0;
+    for (size_t i = 0; i < n_columns; ++i) {
+        B200_CHECK(d_polys[i] && lengths[i] >= 1 && lengths[i] <= N, -1, "evaluate_h_dev: column %zu is null, empty or longer than 2^ext_k", i);
+        const uintptr_t lo = (uintptr_t)d_polys[i], hi = lo + sizeof(Fr) * lengths[i];
+        B200_CHECK(hi <= out_lo || lo >= out_hi, -1, "evaluate_h_dev: d_out overlaps column %zu", i);
+        if (lengths[i] < N) ++n_coeff;
+    }
+    StreamScope ss(c, stream);
+    if (c->stage_c.ensure(sizeof(Fr) * n * (n_coeff ? n_coeff : 1)) || c->stage_b.ensure(sizeof(Fr) * N)) return -2;
+    Fr* h = reinterpret_cast<Fr*>(d_out);
+    if (int rc = evaluate_h_parts_on(c, ss.st, reinterpret_cast<const Fr* const*>(d_polys), lengths, n_columns, k, ext_k, as_fr(ext_omega), as_fr(zeta), loads, n_loads,
+                                     constants, n_constants, program, n_instr, c->stage_c.as<Fr>(), c->stage_b.as<Fr>(), h, nullptr)) return rc;
+    if (!t_evaluations) return 0;
+    return evaluate_h_finish(c, ss.st, h, c->stage_b.as<Fr>(), ext_k, zeta, t_evaluations, t_period, ext_omega_inv, ext_ifft_divisor);
 }
 
 }  // extern "C"

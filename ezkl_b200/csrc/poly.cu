@@ -74,12 +74,14 @@ int poly_scale_cycle(const Fr* a, const Fr* h_consts, uint32_t period, Fr* out, 
     return 0;
 }
 
-// column blockIdx.y: out[s] = sum_{t = s + q n < len} a[t] * cyc[t mod 3] * w^(mul * t mod 2^log_w), s < n.  tab = [cyc[3] | lo | hi] with
-// w^e = lo[e mod 2^lo_bits] * hi[e >> lo_bits].
-__global__ void __launch_bounds__(256) k_poly_coset_fold(const Fr* __restrict__ a_all, size_t a_stride, size_t len, const Fr* __restrict__ tab, uint32_t lo_bits,
+// column y0 + blockIdx.y, cols[.] = (a, len): out[s] = sum_{t = s + q n < len} a[t] * cyc[t mod 3] * w^(mul * t mod 2^log_w), s < n.
+// tab = [cyc[3] | lo | hi] with w^e = lo[e mod 2^lo_bits] * hi[e >> lo_bits].
+__global__ void __launch_bounds__(256) k_poly_coset_fold(const FoldCol* __restrict__ cols, uint32_t y0, const Fr* __restrict__ tab, uint32_t lo_bits,
                                                          uint64_t mul, uint64_t emask, Fr* __restrict__ out_all, size_t out_stride, size_t n) {
-    const Fr* a = a_all + (size_t)blockIdx.y * a_stride;
-    Fr* out = out_all + (size_t)blockIdx.y * out_stride;
+    const size_t y = (size_t)y0 + blockIdx.y;
+    const Fr* a = cols[y].a;
+    const size_t len = cols[y].len;
+    Fr* out = out_all + y * out_stride;
     const Fr* lo = tab + 3;
     const Fr* hi = lo + ((size_t)1 << lo_bits);
     const uint64_t lo_mask = ((uint64_t)1 << lo_bits) - 1;
@@ -93,12 +95,15 @@ __global__ void __launch_bounds__(256) k_poly_coset_fold(const Fr* __restrict__ 
         fp_store(out + s, acc);
     }
 }
-int poly_coset_fold(const Fr* a, size_t a_stride, size_t len, const Fr* d_tab, uint32_t lo_bits, uint32_t log_w, uint64_t mul, Fr* out, size_t out_stride, size_t n,
-                    int batch, cudaStream_t st) {
-    B200_CHECK(batch > 0 && batch <= 65535 && n > 0 && lo_bits <= log_w && log_w <= 28, -1, "poly_coset_fold: bad argument");
-    k_poly_coset_fold<<<dim3(ew_grid(n), batch), 256, 0, st>>>(a, a_stride, len, d_tab, lo_bits, mul, ((uint64_t)1 << log_w) - 1, out, out_stride, n);
-    count_launch();
-    B200_CUDA(cudaGetLastError());
+int poly_coset_fold(const FoldCol* d_cols, size_t n_cols, const Fr* d_tab, uint32_t lo_bits, uint32_t log_w, uint64_t mul, Fr* out, size_t out_stride, size_t n,
+                    cudaStream_t st) {
+    B200_CHECK(n > 0 && n_cols < (1ull << 32) && lo_bits <= log_w && log_w <= 28, -1, "poly_coset_fold: bad argument");
+    for (size_t y0 = 0; y0 < n_cols; y0 += 65535) {          // one launch up to the grid's y limit
+        const unsigned ny = (unsigned)(n_cols - y0 < 65535 ? n_cols - y0 : 65535);
+        k_poly_coset_fold<<<dim3(ew_grid(n), ny), 256, 0, st>>>(d_cols, (uint32_t)y0, d_tab, lo_bits, mul, ((uint64_t)1 << log_w) - 1, out, out_stride, n);
+        count_launch();
+        B200_CUDA(cudaGetLastError());
+    }
     return 0;
 }
 

@@ -16,11 +16,12 @@ int poly_binary(int op, const Fr* a, const Fr* b, const Fr* h_s, Fr* out, size_t
 int poly_lincomb(const Fr* const* h_polys, const Fr* h_scalars, size_t count, Fr* out, size_t n, StagingRing& ring, cudaStream_t st);
 // out[i] = a[i] * consts[i mod period]   (distribute_powers_zeta: period 3; divide_by_vanishing_poly: period 2^(ext_k-k)); h_consts host array
 int poly_scale_cycle(const Fr* a, const Fr* h_consts, uint32_t period, Fr* out, size_t n, StagingRing& ring, cudaStream_t st);
-// one n-point coset part of `batch` coefficient columns a[p * a_stride + t], t < len, before its size-n NTT:
+// one n-point coset part of n_cols coefficient columns before its size-n NTT; d_cols = device table, column p at d_cols[p].a with d_cols[p].len elements:
 // out[p * out_stride + s] = sum_{t = s + q n < len} a[p][t] * g^t for s < n, with g^t = cyc[t mod 3] * w^(mul * t mod 2^log_w).
-// d_tab = [cyc[3] | w^e for e < 2^lo_bits | w^(e << lo_bits) for e < 2^(log_w - lo_bits)], device resident.
-int poly_coset_fold(const Fr* a, size_t a_stride, size_t len, const Fr* d_tab, uint32_t lo_bits, uint32_t log_w, uint64_t mul, Fr* out, size_t out_stride, size_t n,
-                    int batch, cudaStream_t st);
+// d_tab = [cyc[3] | w^e for e < 2^lo_bits | w^(e << lo_bits) for e < 2^(log_w - lo_bits)], device resident.  One launch per 65535 columns.
+struct FoldCol { const Fr* a; uint64_t len; };
+int poly_coset_fold(const FoldCol* d_cols, size_t n_cols, const Fr* d_tab, uint32_t lo_bits, uint32_t log_w, uint64_t mul, Fr* out, size_t out_stride, size_t n,
+                    cudaStream_t st);
 // out[p] = sum_i coeffs[p*stride + i] * x[p]^i   for p < batch (eval_polynomial); h_x host array, d_out device array
 int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_out, int batch, PolyWorkspace& ws, StagingRing& ring, cudaStream_t st);
 // in place a[i] <- a[i]^-1 (zeros stay zero)  (ff::BatchInvert)

@@ -16,9 +16,11 @@
 
 namespace b200 {
 
-struct QLoadDev { const Fr* col; uint32_t offset, pad; };      // 16 B: column pointer resolved on the host
+// 16 B: column pointer resolved on the host; shift != 0 (STRIDED launches only) reads every 2^shift-th element of the column, so one
+// coset part of an extended column is loaded in place: row idx of part c is element c + ((idx + offset) & mask) << shift, col = base + c
+struct QLoadDev { const Fr* col; uint32_t offset, shift; };
 
-template <int NSLOT>
+template <int NSLOT, bool STRIDED>
 __global__ void __launch_bounds__(128) k_quotient_eval(const uint4* __restrict__ blob, uint32_t blob_u4, uint32_t o_loads_u4, uint32_t o_consts_u4, uint32_t mask,
                                                         uint32_t n_instr, Fr* __restrict__ out, uint32_t out_shift, uint32_t out_off) {
     extern __shared__ uint4 sh[];
@@ -37,6 +39,7 @@ __global__ void __launch_bounds__(128) k_quotient_eval(const uint4* __restrict__
         if (k == QSRC_SLOT) return slots[i & (NSLOT - 1)];
         if (k == QSRC_CONST) return fp_load(consts + i);
         const QLoadDev l = loads[i];
+        if (STRIDED) return fp_load(l.col + (((idx + l.offset) & mask) << l.shift));      // < 2^28: the shift is checked on the host
         return fp_load(l.col + ((idx + l.offset) & mask));
     };
 #pragma unroll 1
@@ -61,14 +64,20 @@ __global__ void __launch_bounds__(128) k_quotient_eval(const uint4* __restrict__
     fp_store(out + ((idx << out_shift) + out_off), prev);      // the row's result is the last instruction's (zero for an empty program)
 }
 
-int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k, const QLoad* h_loads, size_t n_loads, const Fr* h_consts, size_t n_consts,
-                      const QInstr* h_prog, size_t n_instr, Fr* d_out, uint32_t out_shift, uint32_t out_off, StagingRing& ring, cudaStream_t st) {
+int quotient_eval_run(const Fr* const* h_col_ptrs, const uint32_t* h_col_shifts, size_t n_cols, uint32_t ext_k, const QLoad* h_loads, size_t n_loads,
+                      const Fr* h_consts, size_t n_consts, const QInstr* h_prog, size_t n_instr, Fr* d_out, uint32_t out_shift, uint32_t out_off, StagingRing& ring,
+                      cudaStream_t st) {
     B200_CHECK(ext_k >= 1 && ext_k <= 28, -1, "quotient_eval: ext_k %u out of range", ext_k);
     B200_CHECK(ext_k + out_shift <= 28 && out_off < (1u << out_shift), -1, "quotient_eval: output layout out of range");
     B200_CHECK(n_instr < (1u << 24) && n_loads < (1u << 30) && n_consts < (1u << 30), -1, "quotient_eval: program too large");
     const uint32_t N = 1u << ext_k;
     // validate the program on the host so the kernel can index without checks
     for (size_t i = 0; i < n_loads; ++i) B200_CHECK(h_loads[i].column < n_cols && h_loads[i].offset < N, -1, "quotient_eval: load %zu out of range", i);
+    bool strided = false;
+    for (size_t i = 0; h_col_shifts && i < n_cols; ++i) {
+        B200_CHECK(ext_k + h_col_shifts[i] <= 28, -1, "quotient_eval: column %zu: stride 2^%u out of range", i, h_col_shifts[i]);
+        strided |= h_col_shifts[i] != 0;
+    }
     uint32_t max_slot = 0;
     for (size_t pc = 0; pc < n_instr; ++pc) {
         const uint32_t op = h_prog[pc].op_dst & 0xff, dst = (h_prog[pc].op_dst >> 8) & 0xffff;
@@ -89,7 +98,7 @@ int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k
     std::vector<uint8_t> blob(total, 0);
     if (n_instr) memcpy(blob.data(), h_prog, sizeof(QInstr) * n_instr);
     for (size_t i = 0; i < n_loads; ++i) {
-        QLoadDev l; l.col = h_col_ptrs[h_loads[i].column]; l.offset = h_loads[i].offset; l.pad = 0;
+        QLoadDev l; l.col = h_col_ptrs[h_loads[i].column]; l.offset = h_loads[i].offset; l.shift = h_col_shifts ? h_col_shifts[h_loads[i].column] : 0;
         memcpy(blob.data() + o_loads + sizeof(QLoadDev) * i, &l, sizeof l);
     }
     if (n_consts) memcpy(blob.data() + o_consts, h_consts, sizeof(Fr) * n_consts);
@@ -99,16 +108,22 @@ int quotient_eval_run(const Fr* const* h_col_ptrs, size_t n_cols, uint32_t ext_k
     const size_t smem = (size_t)blob_u4 * 16;
     const dim3 grid(div_up(N, 128));
     ProfScope ps(PROF_QUOTIENT, st);
-#define B200_QLAUNCH(NS)                                                                                                              \
+#define B200_QLAUNCH(NS, STRIDED)                                                                                                     \
     do {                                                                                                                              \
-        B200_CUDA(cudaFuncSetAttribute(k_quotient_eval<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024 + 64));            \
-        k_quotient_eval<NS><<<grid, 128, smem, st>>>(reinterpret_cast<const uint4*>(d), blob_u4, (uint32_t)(o_loads / 16), (uint32_t)(o_consts / 16), N - 1, \
-                                                     (uint32_t)n_instr, d_out, out_shift, out_off);                                    \
+        B200_CUDA(cudaFuncSetAttribute(k_quotient_eval<NS, STRIDED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024 + 64));   \
+        k_quotient_eval<NS, STRIDED><<<grid, 128, smem, st>>>(reinterpret_cast<const uint4*>(d), blob_u4, (uint32_t)(o_loads / 16), (uint32_t)(o_consts / 16), \
+                                                              N - 1, (uint32_t)n_instr, d_out, out_shift, out_off);                   \
     } while (0)
-    if (max_slot < 32) B200_QLAUNCH(32);
-    else if (max_slot < 64) B200_QLAUNCH(64);
-    else if (max_slot < 128) B200_QLAUNCH(128);
-    else B200_QLAUNCH(256);
+#define B200_QLAUNCH_SLOTS(STRIDED)                   \
+    do {                                              \
+        if (max_slot < 32) B200_QLAUNCH(32, STRIDED);         \
+        else if (max_slot < 64) B200_QLAUNCH(64, STRIDED);    \
+        else if (max_slot < 128) B200_QLAUNCH(128, STRIDED);  \
+        else B200_QLAUNCH(256, STRIDED);                      \
+    } while (0)
+    if (strided) B200_QLAUNCH_SLOTS(true);
+    else B200_QLAUNCH_SLOTS(false);
+#undef B200_QLAUNCH_SLOTS
 #undef B200_QLAUNCH
     count_launch();
     B200_CUDA(cudaGetLastError());

@@ -308,6 +308,32 @@ def evaluate_h_from_polys(program: QuotientProgram, polys, domain, finish: bool 
     return out
 
 
+def evaluate_h_from_polys_device(program: QuotientProgram, polys, domain, finish: bool = False, out=None):
+    """b200_evaluate_h_dev: evaluate_h_from_polys on device-resident columns.  polys = contiguous torch int64 CUDA tensors [len, 4], each in
+    coefficient form (len < 2^ext_k) or extended (len == 2^ext_k); they may be views of one allocation.  Evaluated one n-point coset part at
+    a time with the extended columns read in place (include/ezkl_b200_resident.h); the same bytes as evaluate_h_from_polys.  Enqueued on
+    torch's current stream; returns `out` ([2^ext_k, 4], allocated when None)."""
+    import torch
+    from .device import _stream
+    nat.ensure_init()
+    N = 1 << domain.extended_k
+    for c in polys:
+        assert c.is_cuda and c.dtype == torch.int64 and c.is_contiguous() and c.dim() == 2 and c.shape[1] == 4 and 1 <= c.shape[0] <= N
+    if out is None:
+        out = torch.empty((N, 4), dtype=torch.int64, device="cuda")
+    assert out.is_cuda and out.dtype == torch.int64 and out.is_contiguous() and out.shape == (N, 4)
+    lens = (C.c_size_t * max(1, len(polys)))(*[c.shape[0] for c in polys])
+    ptrs = (C.c_void_p * max(1, len(polys)))(*[c.data_ptr() for c in polys])
+    loads, consts, prog = program.arrays()
+    nat.check(nat.lib().b200_evaluate_h_dev(ptrs if polys else None, lens if polys else None, len(polys), domain.k, domain.extended_k,
+                                            nat.ptr(domain.extended_omega), nat.ptr(domain.g_coset), loads.ctypes.data_as(C.c_void_p), loads.shape[0],
+                                            nat.ptr(consts) if consts.size else None, consts.shape[0], prog.ctypes.data_as(C.c_void_p), prog.shape[0],
+                                            nat.ptr(domain.t_evaluations) if finish else None, domain.t_evaluations.shape[0] if finish else 0,
+                                            nat.ptr(domain.extended_omega_inv) if finish else None, nat.ptr(domain.extended_ifft_divisor) if finish else None,
+                                            out.data_ptr(), _stream()))
+    return out
+
+
 def evaluate_h_device(program: QuotientProgram, columns, k: int, ext_k: int, out=None):
     """Device path: columns = list of torch int64 CUDA tensors [2^ext_k, 4]; enqueued on torch's current stream."""
     import torch
