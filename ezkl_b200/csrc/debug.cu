@@ -1,35 +1,123 @@
 // debug.cu — small self-test entry points (b200_debug_*) used only by tests/ to localise a failure to one layer
 // (field arithmetic, group law, digit recoding) before the composite kernels are blamed.  Not part of the drop-in ABI.
 #include "debug.h"
+#include "ec_coop.cuh"
 #include "msm.cuh"
 #include "ntt.cuh"
 
 namespace b200 {
+// ---- op tables: one HD dispatch function per family, called by the device kernel and by its host twin alike ---------------
+// field ops on Montgomery words: 0 a + b, 1 a - b, 2 a * b, 3 inv(a), 4 from_mont(a), 5 sqr(a), 6 -a, 7 2a, 8 to_mont(a)
 template <class Tag>
-__global__ void k_dbg_field(int op, const Fp<Tag>* a, const Fp<Tag>* b, Fp<Tag>* o, size_t n) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    Fp<Tag> x = fp_load(a + i), y = fp_load(b + i), r;
-    if (op == 0) r = x + y; else if (op == 1) r = x - y; else if (op == 2) r = x * y; else if (op == 3) r = fp_inv(x); else r = fp_from_mont(x);
-    fp_store(o + i, r);
+HD Fp<Tag> dbg_field(int op, const Fp<Tag>& x, const Fp<Tag>& y) {
+    switch (op) {
+        case 0: return x + y;
+        case 1: return x - y;
+        case 2: return x * y;
+        case 3: return fp_inv(x);
+        case 4: return fp_from_mont(x);
+        case 5: return fp_sqr(x);
+        case 6: return fp_neg(x);
+        case 7: return fp_dbl(x);
+        default: return fp_to_mont(x);
+    }
 }
-// op 0: affine a + affine b; 1: 2*a; 2: k*a (k = b.x.l[0] as small integer); 3: a + a via add_mixed (doubling branch); 4: a + (-a)
-__global__ void k_dbg_g1(int op, const G1Affine* a, const G1Affine* b, G1Affine* o, size_t n) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    G1Affine p = a[i], q = b[i];
+// two-product ops: 0 a b + c d (fp_muladd2), 1 a b - c d (fp_mulsub2)
+template <class Tag>
+HD Fp<Tag> dbg_field4(int op, const Fp<Tag>& a, const Fp<Tag>& b, const Fp<Tag>& c, const Fp<Tag>& d) {
+    return op == 0 ? fp_muladd2(a, b, c, d) : fp_mulsub2(a, b, c, d);
+}
+// affine in, affine out.  op 0: a + b; 1: 2a; 2: k a (k = b.x.l[0] as small integer); 3: a + 2b via g1_add (doubling branch when
+// a == 2b); 4: a + (-a)
+HD G1Affine dbg_g1(int op, const G1Affine& p, const G1Affine& q) {
     G1Xyzz r;
     if (op == 0) r = g1_add_mixed(g1_to_xyzz(p), q);
     else if (op == 1) r = g1_dbl(g1_to_xyzz(p));
     else if (op == 2) r = g1_mul_small(g1_to_xyzz(p), q.x.l[0]);
     else if (op == 3) r = g1_add(g1_to_xyzz(p), g1_dbl_affine(q));
     else r = g1_add_mixed(g1_to_xyzz(p), g1_neg(p));
-    o[i] = g1_to_affine(r);
+    return g1_to_affine(r);
+}
+// XYZZ in, raw XYZZ words out (no normalisation).  op 0: g1_add(a, b); 1: g1_dbl(a); 2: g1_add_mixed(a, (b.x, b.y)); 3: g1_mul_small(a, k);
+// 4: g1_to_affine(a) as (x, y, 0, 0); 5: g1_add_coop4(a, b) and 6: g1_dbl_coop4(a), device only (DBG_XYZZ_COOP and above).
+enum { DBG_XYZZ_COOP = 5 };
+HD G1Xyzz dbg_xyzz(int op, const G1Xyzz& a, const G1Xyzz& b, uint32_t k) {
+    switch (op) {
+        case 0: return g1_add(a, b);
+        case 1: return g1_dbl(a);
+        case 2: { G1Affine q; q.x = b.x; q.y = b.y; return g1_add_mixed(a, q); }
+        case 3: return g1_mul_small(a, k);
+        default: {
+            const G1Affine q = g1_to_affine(a);
+            G1Xyzz r = g1_xyzz_identity(); r.x = q.x; r.y = q.y;
+            return r;
+        }
+    }
+}
+
+template <class Tag>
+__global__ void k_dbg_field(int op, const Fp<Tag>* a, const Fp<Tag>* b, Fp<Tag>* o, size_t n) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) fp_store(o + i, dbg_field(op, fp_load(a + i), fp_load(b + i)));
+}
+template <class Tag>
+__global__ void k_dbg_field4(int op, const Fp<Tag>* a, const Fp<Tag>* b, const Fp<Tag>* c, const Fp<Tag>* d, Fp<Tag>* o, size_t n) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) fp_store(o + i, dbg_field4(op, fp_load(a + i), fp_load(b + i), fp_load(c + i), fp_load(d + i)));
+}
+__global__ void k_dbg_g1(int op, const G1Affine* a, const G1Affine* b, G1Affine* o, size_t n) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) o[i] = dbg_g1(op, a[i], b[i]);
+}
+// one element per thread; the cooperative ops take one element per quad (all four lanes load it, lane 0 writes), so consecutive
+// elements are neighbouring quads of one warp and may take different branches
+__global__ void k_dbg_xyzz(int op, const G1Xyzz* a, const G1Xyzz* b, const uint32_t* k, G1Xyzz* o, size_t n) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (op >= DBG_XYZZ_COOP) {
+        const size_t i = t >> 2;
+        if (i >= n) return;                 // a whole quad leaves together
+        const G1Xyzz r = op == DBG_XYZZ_COOP ? g1_add_coop4(a[i], b[i]) : g1_dbl_coop4(a[i]);
+        if ((t & 3) == 0) o[i] = r;
+        return;
+    }
+    if (t < n) o[t] = dbg_xyzz(op, a[t], b[t], k[t]);
 }
 __global__ void k_dbg_xyzz_to_affine(const G1Xyzz* p, G1Affine* o, size_t n) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) o[i] = g1_to_affine(p[i]);
 }
+// host twins' loops over the field op tables
+template <class Tag> static void host_field_op(int op, const b200_fr* a, const b200_fr* b, b200_fr* out, size_t n) {
+    for (size_t i = 0; i < n; ++i) {
+        Fp<Tag> x, y; memcpy(&x, &a[i], 32); memcpy(&y, &b[i], 32);
+        const Fp<Tag> r = dbg_field(op, x, y); memcpy(&out[i], &r, 32);
+    }
+}
+template <class Tag> static void host_field_op4(int op, const b200_fr* a, const b200_fr* b, const b200_fr* c, const b200_fr* d, b200_fr* out, size_t n) {
+    for (size_t i = 0; i < n; ++i) {
+        Fp<Tag> w, x, y, z; memcpy(&w, &a[i], 32); memcpy(&x, &b[i], 32); memcpy(&y, &c[i], 32); memcpy(&z, &d[i], 32);
+        const Fp<Tag> r = dbg_field4(op, w, x, y, z); memcpy(&out[i], &r, 32);
+    }
+}
+// device copies of the HOST arrays of one debug call, freed when the call returns on any path
+struct DbgStage {
+    DevBuf bufs[6];
+    int used = 0;
+    template <class T> int in(const void* src, size_t bytes, T** d) {
+        DevBuf& b = bufs[used++];
+        if (b.ensure(bytes ? bytes : 1)) return -2;
+        B200_CUDA(cudaMemcpy(b.p, src, bytes, cudaMemcpyHostToDevice));
+        *d = b.as<T>();
+        return 0;
+    }
+    template <class T> int out(size_t bytes, T** d) {
+        DevBuf& b = bufs[used++];
+        if (b.ensure(bytes ? bytes : 1)) return -2;
+        *d = b.as<T>();
+        return 0;
+    }
+    ~DbgStage() { for (DevBuf& b : bufs) b.release(); }
+};
 // What msm.cu (linked into this library for b200_debug_msm_base_off) needs from the product's capi.cu: default tuning, the SM count,
 // and no event profiling.
 static Config g_dbg_cfg;
@@ -130,24 +218,59 @@ using namespace b200;
 extern "C" {
 // all pointers are HOST pointers; the call stages, runs one kernel and copies back
 int b200_debug_field_op(int field, int op, const b200_fr* a, const b200_fr* b, b200_fr* out, size_t n) {
-    void *da, *db, *dout;
-    B200_CUDA(cudaMalloc(&da, 32 * n)); B200_CUDA(cudaMalloc(&db, 32 * n)); B200_CUDA(cudaMalloc(&dout, 32 * n));
-    B200_CUDA(cudaMemcpy(da, a, 32 * n, cudaMemcpyHostToDevice)); B200_CUDA(cudaMemcpy(db, b, 32 * n, cudaMemcpyHostToDevice));
-    if (field == 0) k_dbg_field<FrTag><<<div_up(n, 128), 128>>>(op, (const Fr*)da, (const Fr*)db, (Fr*)dout, n);
+    if (n == 0) return 0;
+    DbgStage st;
+    Fr *da, *db, *dout;
+    if (int rc = st.in(a, 32 * n, &da)) return rc;
+    if (int rc = st.in(b, 32 * n, &db)) return rc;
+    if (int rc = st.out(32 * n, &dout)) return rc;
+    if (field == 0) k_dbg_field<FrTag><<<div_up(n, 128), 128>>>(op, da, db, dout, n);
     else k_dbg_field<FqTag><<<div_up(n, 128), 128>>>(op, (const Fq*)da, (const Fq*)db, (Fq*)dout, n);
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpy(out, dout, 32 * n, cudaMemcpyDeviceToHost));
-    cudaFree(da); cudaFree(db); cudaFree(dout);
+    return 0;
+}
+int b200_debug_field_op4(int field, int op, const b200_fr* a, const b200_fr* b, const b200_fr* c, const b200_fr* d, b200_fr* out, size_t n) {
+    if (n == 0) return 0;
+    DbgStage st;
+    Fr *da, *db, *dc, *dd, *dout;
+    if (int rc = st.in(a, 32 * n, &da)) return rc;
+    if (int rc = st.in(b, 32 * n, &db)) return rc;
+    if (int rc = st.in(c, 32 * n, &dc)) return rc;
+    if (int rc = st.in(d, 32 * n, &dd)) return rc;
+    if (int rc = st.out(32 * n, &dout)) return rc;
+    if (field == 0) k_dbg_field4<FrTag><<<div_up(n, 128), 128>>>(op, da, db, dc, dd, dout, n);
+    else k_dbg_field4<FqTag><<<div_up(n, 128), 128>>>(op, (const Fq*)da, (const Fq*)db, (const Fq*)dc, (const Fq*)dd, (Fq*)dout, n);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpy(out, dout, 32 * n, cudaMemcpyDeviceToHost));
     return 0;
 }
 int b200_debug_g1_op(int op, const b200_g1_affine* a, const b200_g1_affine* b, b200_g1_affine* out, size_t n) {
-    void *da, *db, *dout;
-    B200_CUDA(cudaMalloc(&da, 64 * n)); B200_CUDA(cudaMalloc(&db, 64 * n)); B200_CUDA(cudaMalloc(&dout, 64 * n));
-    B200_CUDA(cudaMemcpy(da, a, 64 * n, cudaMemcpyHostToDevice)); B200_CUDA(cudaMemcpy(db, b, 64 * n, cudaMemcpyHostToDevice));
-    k_dbg_g1<<<div_up(n, 64), 64>>>(op, (const G1Affine*)da, (const G1Affine*)db, (G1Affine*)dout, n);
+    if (n == 0) return 0;
+    DbgStage st;
+    G1Affine *da, *db, *dout;
+    if (int rc = st.in(a, 64 * n, &da)) return rc;
+    if (int rc = st.in(b, 64 * n, &db)) return rc;
+    if (int rc = st.out(64 * n, &dout)) return rc;
+    k_dbg_g1<<<div_up(n, 64), 64>>>(op, da, db, dout, n);
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpy(out, dout, 64 * n, cudaMemcpyDeviceToHost));
-    cudaFree(da); cudaFree(db); cudaFree(dout);
+    return 0;
+}
+int b200_debug_g1_xyzz_op(int op, const b200_g1_xyzz* a, const b200_g1_xyzz* b, const uint32_t* k, b200_g1_xyzz* out, size_t n) {
+    if (op < 0 || op > DBG_XYZZ_COOP + 1) return -1;
+    if (n == 0) return 0;
+    DbgStage st;
+    G1Xyzz *da, *db, *dout;
+    uint32_t* dk;
+    if (int rc = st.in(a, 128 * n, &da)) return rc;
+    if (int rc = st.in(b, 128 * n, &db)) return rc;
+    if (int rc = st.in(k, 4 * n, &dk)) return rc;
+    if (int rc = st.out(128 * n, &dout)) return rc;
+    const size_t threads = op >= DBG_XYZZ_COOP ? 4 * n : n;
+    k_dbg_xyzz<<<div_up(threads, 64), 64>>>(op, da, db, dk, dout, n);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpy(out, dout, 128 * n, cudaMemcpyDeviceToHost));
     return 0;
 }
 int b200_debug_digits(const b200_fr* s, size_t n, int c, int32_t* out /* n * ceil(255/c) */) {
@@ -288,30 +411,29 @@ int b200_debug_ntt_plan_host(uint32_t log_n, int batch, int sm_count, int64_t* o
     }
     return npass;
 }
-// host-only: group law / field code compiled for the CPU through the portable path (not-gpu tests)
+// host-only twins of the calls above: the same op tables compiled for the CPU, through the portable path (not-gpu tests and
+// the host tail, normalize_host, run this code)
 int b200_debug_host_g1_op(int op, const b200_g1_affine* a, const b200_g1_affine* b, b200_g1_affine* out, size_t n) {
     for (size_t i = 0; i < n; ++i) {
         G1Affine p, q; memcpy(&p, &a[i], 64); memcpy(&q, &b[i], 64);
-        G1Xyzz r;
-        if (op == 0) r = g1_add_mixed(g1_to_xyzz(p), q);
-        else if (op == 1) r = g1_dbl(g1_to_xyzz(p));
-        else if (op == 2) r = g1_mul_small(g1_to_xyzz(p), q.x.l[0]);
-        else if (op == 3) r = g1_add(g1_to_xyzz(p), g1_dbl_affine(q));
-        else r = g1_add_mixed(g1_to_xyzz(p), g1_neg(p));
-        G1Affine o = g1_to_affine(r); memcpy(&out[i], &o, 64);
+        const G1Affine o = dbg_g1(op, p, q); memcpy(&out[i], &o, 64);
+    }
+    return 0;
+}
+int b200_debug_host_g1_xyzz_op(int op, const b200_g1_xyzz* a, const b200_g1_xyzz* b, const uint32_t* k, b200_g1_xyzz* out, size_t n) {
+    if (op < 0 || op >= DBG_XYZZ_COOP) return -1;           // the cooperative ops exist on the device only
+    for (size_t i = 0; i < n; ++i) {
+        G1Xyzz p, q; memcpy(&p, &a[i], 128); memcpy(&q, &b[i], 128);
+        const G1Xyzz o = dbg_xyzz(op, p, q, k[i]); memcpy(&out[i], &o, 128);
     }
     return 0;
 }
 int b200_debug_host_field_op(int field, int op, const b200_fr* a, const b200_fr* b, b200_fr* out, size_t n) {
-    for (size_t i = 0; i < n; ++i) {
-        if (field == 0) { Fr x, y, r; memcpy(&x, &a[i], 32); memcpy(&y, &b[i], 32);
-            if (op == 0) r = x + y; else if (op == 1) r = x - y; else if (op == 2) r = x * y; else if (op == 3) r = fp_inv(x); else r = fp_from_mont(x);
-            memcpy(&out[i], &r, 32);
-        } else { Fq x, y, r; memcpy(&x, &a[i], 32); memcpy(&y, &b[i], 32);
-            if (op == 0) r = x + y; else if (op == 1) r = x - y; else if (op == 2) r = x * y; else if (op == 3) r = fp_inv(x); else r = fp_from_mont(x);
-            memcpy(&out[i], &r, 32);
-        }
-    }
+    if (field == 0) host_field_op<FrTag>(op, a, b, out, n); else host_field_op<FqTag>(op, a, b, out, n);
+    return 0;
+}
+int b200_debug_host_field_op4(int field, int op, const b200_fr* a, const b200_fr* b, const b200_fr* c, const b200_fr* d, b200_fr* out, size_t n) {
+    if (field == 0) host_field_op4<FrTag>(op, a, b, c, d, out, n); else host_field_op4<FqTag>(op, a, b, c, d, out, n);
     return 0;
 }
 }
