@@ -1266,148 +1266,79 @@ int b200_quotient_eval(const b200_fr* const* columns, size_t n_columns, uint32_t
     return d2h_one(c, out, c->stage_b.p, sizeof(Fr) * N, ss.st);
 }
 
-// evaluate_h with every column's extended coset resident: stage_c = the cosets, stage_a = coefficient staging (one sub-batch),
-// stage_b = NTT scratch / output.  On return h = stage_b[0, N) and stage_c is free.
-static int evaluate_h_cosets(Ctx* c, cudaStream_t st, const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
-                             const b200_fr* ext_omega, const b200_fr* zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
-                             const b200_instr* program, size_t n_instr) {
-    const size_t N = (size_t)1 << ext_k;
-    if (c->stage_c.ensure(sizeof(Fr) * N * (n_columns ? n_columns : 1))) return -2;
-    size_t n_coeff_cols = 0, max_len = 0;
-    for (size_t i = 0; i < n_columns; ++i) if (lengths[i] < N) { ++n_coeff_cols; if (lengths[i] > max_len) max_len = lengths[i]; }
-    size_t sub = n_coeff_cols ? call_budget() / (sizeof(Fr) * (N + max_len)) : 1;
-    if (sub < 1) sub = 1;
-    if (sub > n_coeff_cols) sub = n_coeff_cols ? n_coeff_cols : 1;
-    if (c->stage_a.ensure(sizeof(Fr) * (max_len ? max_len : 1) * sub) || c->stage_b.ensure(sizeof(Fr) * N * sub)) return -2;
-    Fr* ext = c->stage_c.as<Fr>();
-    NttScale pre, none;
-    pre.mode = 3; pre.c[0] = fp_one<FrTag>(); pre.c[1] = as_fr(zeta); pre.c[2] = as_fr(zeta) * as_fr(zeta);
-    std::vector<size_t> group;           // coefficient columns of equal length are transformed together
-    auto flush = [&](size_t len) -> int {
-        if (group.empty()) return 0;
-        std::vector<HostSeg> up(group.size());
-        for (size_t p = 0; p < group.size(); ++p) up[p] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[group[p]]), sizeof(Fr) * len};
-        if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), st)) return rc;
-        // transform into scratch-free destinations: each polynomial lands in its own column of `ext` (dst stride = distance between them is
-        // irregular, so one launch per run of consecutive column indices)
-        size_t p0 = 0;
-        while (p0 < group.size()) {
-            size_t p1 = p0 + 1;
-            while (p1 < group.size() && group[p1] == group[p1 - 1] + 1) ++p1;
-            if (int rc = ntt_call(c, st, c->stage_a.as<Fr>() + p0 * len, len, len, c->stage_b.as<Fr>(), ext + group[p0] * N, N, ext_k, as_fr(ext_omega), pre, none, (int)(p1 - p0))) return rc;
-            p0 = p1;
-        }
-        B200_CUDA(cudaStreamSynchronize(st));          // the coefficient staging buffer is reused by the next group
-        group.clear();
-        return 0;
-    };
-    size_t cur_len = 0;
-    for (size_t i = 0; i < n_columns; ++i) {
-        if (lengths[i] == N) { if (int rc = h2d_one(c, ext + i * N, polys[i], sizeof(Fr) * N, st)) return rc; continue; }
-        if (!group.empty() && (lengths[i] != cur_len || group.size() == sub)) { if (int rc = flush(cur_len)) return rc; }
-        cur_len = lengths[i];
-        group.push_back(i);
-    }
-    if (int rc = flush(cur_len)) return rc;
-    std::vector<const void*> ptrs(n_columns);
-    for (size_t i = 0; i < n_columns; ++i) ptrs[i] = ext + i * N;
-    return quotient_eval_on(c, st, ptrs.data(), n_columns, k, ext_k, loads, n_loads, constants, n_constants, program, n_instr, c->stage_b.p);
-}
-
-// evaluate_h by parts: the extended domain of N = d n points is the disjoint union of the d cosets of the n-point domain; part c
-// holds the extended indices c + d i (the points g_c w_n^i, g_c = zeta w_N^c).  A rotation by r rows moves c + d i to
-// c + d ((i + r) mod n), inside part c, so the numerator on part c reads only part c of every column: n elements per column.  Per part:
-//   coefficient columns: part c of column p is the size-n NTT (w_n = w_N^d) of b_s = sum_q p_{s+qn} g_c^{s+qn}, folded and pre-scaled
+// evaluate_h by parts: for any p <= ext_k - k the extended domain of N = 2^ext_k points is the disjoint union of P = 2^p cosets of
+// m = N / P points; part c holds the extended indices c + P i (the points g_c w_m^i, g_c = zeta w_N^c, w_m = w_N^P).  A rotation by r
+// rows moves an index by r 2^(ext_k - k), a multiple of P, so it stays inside part c: the numerator on part c reads only part c of every
+// column, m elements per column.  p = 0 is one part, the whole extended coset; p = ext_k - k is 2^(ext_k - k) parts of n points.  Per part:
+//   coefficient columns: p = 0: the size-N coset NTT of each column from its coefficients (pre-scaled by [1, zeta, zeta^2], n_in = its
+//                        length, so the transform skips the zero padding), one column per transform (tmp holds one coset);
+//                        p > 0: part c of column q is the size-m NTT (w_m) of b_s = sum_j q_{s+jm} g_c^{s+jm}, folded and pre-scaled
 //                        by ONE poly_coset_fold launch for every coefficient column (a device table of (address, length) per column) from
-//                        two small power tables of w_N, then transformed in batches of at most d columns (tmp holds d parts);
-//   extended columns:    read in place by the interpreter, elements c, c + d, c + 2d, ... of cols[i] (a load of stride d from cols[i] + c);
-//                        or, when stage_ext is given, staged by stage_ext(c) as n contiguous elements at cols[i] and read densely;
-//   numerator:           the interpreter at (k, k), storing row i at index c + d i of h.
-// cols[i] = device address of column i, lengths[i] < N: coefficient form, == N: extended.  Device memory: parts = n_coeff * n elements (the
-// coefficient columns' parts, in column order), tmp = N elements, and the power and fold tables in c->small.  Both evaluate_h entry points
-// run this loop: the host one on columns it uploads, the _dev one on the caller's.
-static int evaluate_h_parts_on(Ctx* c, cudaStream_t st, const Fr* const* cols, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
+//                        two small power tables of w_N, then transformed in batches of at most P columns (tmp holds P parts);
+//   extended columns:    read in place by the interpreter, elements c, c + P, c + 2P, ... of cols[i] (a load of stride P from cols[i] + c);
+//                        or, when stage_ext is given, staged by stage_ext(c) as m contiguous elements at cols[i] and read densely;
+//   numerator:           the interpreter on m rows (rotations scale by 2^(ext_k - p - k), wrap mod m), storing row i at index c + P i of h.
+// cols[i] = device address of column i, lengths[i] < N: coefficient form, == N: extended.  Device memory: parts = n_coeff * m elements (the
+// coefficient columns' parts, in column order), tmp = N elements, and for p > 0 the power and fold tables in c->small.  Both evaluate_h
+// entry points run this loop: the host one on columns it uploads, the _dev one on the caller's.
+static int evaluate_h_parts_on(Ctx* c, cudaStream_t st, const Fr* const* cols, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k, uint32_t p,
                                const Fr& ext_omega, const Fr& zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
                                const b200_instr* program, size_t n_instr, Fr* parts, Fr* tmp, Fr* h, const std::function<int(size_t)>& stage_ext) {
-    const size_t N = (size_t)1 << ext_k, n = (size_t)1 << k, d = N >> k;
+    const size_t N = (size_t)1 << ext_k, P = (size_t)1 << p, m = N >> p;
     std::vector<FoldCol> fold;
     for (size_t i = 0; i < n_columns; ++i) if (lengths[i] < N) fold.push_back(FoldCol{cols[i], lengths[i]});
     const uint32_t lo_bits = (ext_k + 1) / 2;
-    const size_t n_lo = (size_t)1 << lo_bits, n_hi = N >> lo_bits, n_tab = 3 + n_lo + n_hi;
-    // [1, zeta, zeta^2 | w_N^e, e < n_lo | w_N^(e n_lo), e < n_hi | the fold table], staged once for every part
-    const size_t tab_bytes = sizeof(Fr) * n_tab, fold_bytes = sizeof(FoldCol) * fold.size();
-    if (c->small.ensure(tab_bytes + fold_bytes)) return -2;
-    std::vector<uint8_t> blob(tab_bytes + fold_bytes);
-    Fr* tab = reinterpret_cast<Fr*>(blob.data());
-    tab[0] = fp_one<FrTag>(); tab[1] = zeta; tab[2] = zeta * zeta;
-    Fr* lo = tab + 3;
-    Fr* hi = lo + n_lo;
-    lo[0] = fp_one<FrTag>();
-    for (size_t e = 1; e < n_lo; ++e) lo[e] = lo[e - 1] * ext_omega;
-    const Fr step = lo[n_lo - 1] * ext_omega;
-    hi[0] = fp_one<FrTag>();
-    for (size_t e = 1; e < n_hi; ++e) hi[e] = hi[e - 1] * step;
-    if (fold_bytes) memcpy(blob.data() + tab_bytes, fold.data(), fold_bytes);
-    if (int rc = ring_upload(c, c->small.p, blob.data(), blob.size(), st)) return rc;
-    const Fr* d_tab = c->small.as<Fr>();
-    const FoldCol* d_fold = reinterpret_cast<const FoldCol*>(c->small.as<uint8_t>() + tab_bytes);
-    Fr omega_n = ext_omega;
-    for (uint32_t i = k; i < ext_k; ++i) omega_n = omega_n * omega_n;
+    const Fr* d_tab = nullptr;
+    const FoldCol* d_fold = nullptr;
+    if (p > 0 && !fold.empty()) {
+        const size_t n_lo = (size_t)1 << lo_bits, n_hi = N >> lo_bits, n_tab = 3 + n_lo + n_hi;
+        // [1, zeta, zeta^2 | w_N^e, e < n_lo | w_N^(e n_lo), e < n_hi | the fold table], staged once for every part
+        const size_t tab_bytes = sizeof(Fr) * n_tab, fold_bytes = sizeof(FoldCol) * fold.size();
+        if (c->small.ensure(tab_bytes + fold_bytes)) return -2;
+        std::vector<uint8_t> blob(tab_bytes + fold_bytes);
+        Fr* tab = reinterpret_cast<Fr*>(blob.data());
+        tab[0] = fp_one<FrTag>(); tab[1] = zeta; tab[2] = zeta * zeta;
+        Fr* lo = tab + 3;
+        Fr* hi = lo + n_lo;
+        lo[0] = fp_one<FrTag>();
+        for (size_t e = 1; e < n_lo; ++e) lo[e] = lo[e - 1] * ext_omega;
+        const Fr step = lo[n_lo - 1] * ext_omega;
+        hi[0] = fp_one<FrTag>();
+        for (size_t e = 1; e < n_hi; ++e) hi[e] = hi[e - 1] * step;
+        memcpy(blob.data() + tab_bytes, fold.data(), fold_bytes);
+        if (int rc = ring_upload(c, c->small.p, blob.data(), blob.size(), st)) return rc;
+        d_tab = c->small.as<Fr>();
+        d_fold = reinterpret_cast<const FoldCol*>(c->small.as<uint8_t>() + tab_bytes);
+    }
+    Fr omega_m = ext_omega;
+    for (uint32_t i = 0; i < p; ++i) omega_m = omega_m * omega_m;
     std::vector<const void*> ptrs(n_columns);
     std::vector<uint32_t> shifts(n_columns, 0);
-    for (size_t i = 0, j = 0; i < n_columns; ++i) if (lengths[i] < N) ptrs[i] = parts + n * j++;
-    NttScale none;
-    for (size_t part = 0; part < d; ++part) {
-        if (!fold.empty()) {
-            if (int rc = poly_coset_fold(d_fold, fold.size(), d_tab, lo_bits, ext_k, part, parts, n, n, st)) return rc;
-            for (size_t j0 = 0; j0 < fold.size(); j0 += d) {
-                const int nb = (int)(fold.size() - j0 < d ? fold.size() - j0 : d);
-                if (int rc = ntt_call(c, st, parts + j0 * n, n, n, tmp, parts + j0 * n, n, k, omega_n, none, none, nb)) return rc;
+    for (size_t i = 0, j = 0; i < n_columns; ++i) if (lengths[i] < N) ptrs[i] = parts + m * j++;
+    NttScale zeta_cycle, none;
+    zeta_cycle.mode = 3; zeta_cycle.c[0] = fp_one<FrTag>(); zeta_cycle.c[1] = zeta; zeta_cycle.c[2] = zeta * zeta;
+    for (size_t part = 0; part < P; ++part) {
+        if (p == 0) {
+            for (size_t j = 0; j < fold.size(); ++j) {
+                const size_t len = fold[j].len;
+                if (int rc = ntt_call(c, st, fold[j].a, len, len, tmp, parts + j * m, m, ext_k, ext_omega, zeta_cycle, none, 1)) return rc;
+            }
+        } else if (!fold.empty()) {
+            if (int rc = poly_coset_fold(d_fold, fold.size(), d_tab, lo_bits, ext_k, part, parts, m, m, st)) return rc;
+            for (size_t j0 = 0; j0 < fold.size(); j0 += P) {
+                const int nb = (int)(fold.size() - j0 < P ? fold.size() - j0 : P);
+                if (int rc = ntt_call(c, st, parts + j0 * m, m, m, tmp, parts + j0 * m, m, ext_k - p, omega_m, none, none, nb)) return rc;
             }
         }
         if (stage_ext) { if (int rc = stage_ext(part)) return rc; }
         for (size_t i = 0; i < n_columns; ++i) if (lengths[i] == N) {
             ptrs[i] = stage_ext ? cols[i] : cols[i] + part;
-            shifts[i] = stage_ext ? 0 : ext_k - k;
+            shifts[i] = stage_ext ? 0 : p;
         }
-        if (int rc = quotient_eval_on(c, st, ptrs.data(), n_columns, k, k, loads, n_loads, constants, n_constants, program, n_instr, h, ext_k - k, (uint32_t)part,
+        if (int rc = quotient_eval_on(c, st, ptrs.data(), n_columns, k, ext_k - p, loads, n_loads, constants, n_constants, program, n_instr, h, p, (uint32_t)part,
                                       shifts.data())) return rc;
     }
     return 0;
-}
-// the host entry point's parts path: stage_a = the coefficient columns (uploaded once), stage_c = n-element parts of every column (the
-// coefficient columns' in column order, then the extended columns', gathered on the host into the pinned bounce slots per part),
-// stage_b = h and an N-element NTT scratch.  On return h = stage_b[0, N) and stage_b[N, 2N) is free.
-static int evaluate_h_parts(Ctx* c, cudaStream_t st, const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
-                            const Fr& ext_omega, const Fr& zeta, const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
-                            const b200_instr* program, size_t n_instr) {
-    const size_t N = (size_t)1 << ext_k, n = (size_t)1 << k, d = N >> k;
-    std::vector<size_t> coeff, exts;
-    size_t coeff_elems = 0;
-    for (size_t i = 0; i < n_columns; ++i) {
-        if (lengths[i] < N) { coeff.push_back(i); coeff_elems += lengths[i]; }
-        else exts.push_back(i);
-    }
-    if (c->stage_c.ensure(sizeof(Fr) * n * n_columns) || c->stage_a.ensure(sizeof(Fr) * (coeff_elems ? coeff_elems : 1)) || c->stage_b.ensure(sizeof(Fr) * 2 * N)) return -2;
-    Fr* parts = c->stage_c.as<Fr>();
-    Fr* h = c->stage_b.as<Fr>();
-    std::vector<HostSeg> up(coeff.size()), ext_up(exts.size());
-    std::vector<const Fr*> cols(n_columns);
-    size_t off = 0;
-    for (size_t j = 0; j < coeff.size(); ++j) {
-        up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[coeff[j]]), sizeof(Fr) * lengths[coeff[j]]};
-        cols[coeff[j]] = c->stage_a.as<Fr>() + off;
-        off += lengths[coeff[j]];
-    }
-    for (size_t j = 0; j < exts.size(); ++j) cols[exts[j]] = parts + (coeff.size() + j) * n;
-    if (!coeff.empty()) { if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), st)) return rc; }
-    auto stage_ext = [&](size_t part) -> int {
-        if (exts.empty()) return 0;
-        for (size_t j = 0; j < exts.size(); ++j) ext_up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[exts[j]] + part), sizeof(Fr) * n, d > 1 ? sizeof(Fr) * d : 0};
-        return h2d_segments(c, parts + coeff.size() * n, ext_up.data(), ext_up.size(), st);
-    };
-    return evaluate_h_parts_on(c, st, cols.data(), lengths, n_columns, k, ext_k, ext_omega, zeta, loads, n_loads, constants, n_constants, program, n_instr,
-                               parts, h + N, h, stage_ext);
 }
 // the finishing step of both evaluate_h entry points, in place in h: h * t_evaluations[i mod t_period], then extended_to_coeff (scratch: N elements)
 static int evaluate_h_finish(Ctx* c, cudaStream_t st, Fr* h, Fr* scratch, uint32_t ext_k, const b200_fr* zeta, const b200_fr* t_evaluations, uint32_t t_period,
@@ -1423,8 +1354,11 @@ static int evaluate_h_finish(Ctx* c, cudaStream_t st, Fr* h, Fr* scratch, uint32
 // evaluate_h at its natural boundary: the CPU evaluator receives coefficient-form polynomials and builds their cosets itself
 // (UPSTREAM plonk/evaluation.rs: `advice_polys.iter().map(|a| domain.coeff_to_extended(a))`), and vanishing/prover.rs then divides by
 // the vanishing polynomial and converts back.  One call does the same on the device, so a coefficient column crosses PCIe once
-// (n elements) instead of its coset twice (2^ext_k down, 2^ext_k up).  When every column's extended coset fits the call budget they
-// are all resident at once; otherwise the numerator is evaluated one n-point coset part at a time (evaluate_h_parts).
+// (n elements) instead of its coset twice (2^ext_k down, 2^ext_k up).  When every column's extended coset fits the call budget the
+// loop runs one part, the whole coset of every column (p = 0); otherwise the numerator is evaluated one n-point coset part at a time
+// (p = ext_k - k).  Device memory: stage_a = the coefficient columns (uploaded once), stage_c = the current m = 2^(ext_k - p) element part
+// of every column (the coefficient columns' in column order, then the extended columns', gathered on the host into the pinned bounce
+// slots per part), stage_b = h (N elements) followed by the N-element NTT scratch of the loop and of the finishing step.
 int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta,
                     const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr,
                     const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, b200_fr* out) {
@@ -1436,19 +1370,36 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
     for (size_t i = 0; i < n_columns; ++i)
         B200_CHECK(polys[i] && lengths[i] >= 1 && lengths[i] <= N, -1, "evaluate_h: column %zu is null or longer than 2^ext_k", i);
     StreamScope ss(c, nullptr);
-    Fr* h = nullptr;
-    Fr* scratch = nullptr;
-    if (k >= 1 && sizeof(Fr) * N * n_columns > call_budget()) {
-        if (int rc = evaluate_h_parts(c, ss.st, polys, lengths, n_columns, k, ext_k, as_fr(ext_omega), as_fr(zeta), loads, n_loads, constants, n_constants, program, n_instr)) return rc;
-        h = c->stage_b.as<Fr>();
-        scratch = h + N;
-    } else {
-        if (int rc = evaluate_h_cosets(c, ss.st, polys, lengths, n_columns, k, ext_k, ext_omega, zeta, loads, n_loads, constants, n_constants, program, n_instr)) return rc;
-        h = c->stage_b.as<Fr>();
-        scratch = c->stage_c.as<Fr>();
+    const uint32_t p = k >= 1 && sizeof(Fr) * N * n_columns > call_budget() ? ext_k - k : 0;
+    const size_t m = N >> p, P = (size_t)1 << p;
+    std::vector<size_t> coeff, exts;
+    size_t coeff_elems = 0;
+    for (size_t i = 0; i < n_columns; ++i) {
+        if (lengths[i] < N) { coeff.push_back(i); coeff_elems += lengths[i]; }
+        else exts.push_back(i);
     }
+    if (c->stage_c.ensure(sizeof(Fr) * m * n_columns) || c->stage_a.ensure(sizeof(Fr) * (coeff_elems ? coeff_elems : 1)) || c->stage_b.ensure(sizeof(Fr) * 2 * N)) return -2;
+    Fr* parts = c->stage_c.as<Fr>();
+    Fr* h = c->stage_b.as<Fr>();
+    std::vector<HostSeg> up(coeff.size()), ext_up(exts.size());
+    std::vector<const Fr*> cols(n_columns);
+    size_t off = 0;
+    for (size_t j = 0; j < coeff.size(); ++j) {
+        up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[coeff[j]]), sizeof(Fr) * lengths[coeff[j]]};
+        cols[coeff[j]] = c->stage_a.as<Fr>() + off;
+        off += lengths[coeff[j]];
+    }
+    for (size_t j = 0; j < exts.size(); ++j) cols[exts[j]] = parts + (coeff.size() + j) * m;
+    if (!coeff.empty()) { if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), ss.st)) return rc; }
+    auto stage_ext = [&](size_t part) -> int {
+        if (exts.empty()) return 0;
+        for (size_t j = 0; j < exts.size(); ++j) ext_up[j] = HostSeg{(uint8_t*)const_cast<b200_fr*>(polys[exts[j]] + part), sizeof(Fr) * m, P > 1 ? sizeof(Fr) * P : 0};
+        return h2d_segments(c, parts + coeff.size() * m, ext_up.data(), ext_up.size(), ss.st);
+    };
+    if (int rc = evaluate_h_parts_on(c, ss.st, cols.data(), lengths, n_columns, k, ext_k, p, as_fr(ext_omega), as_fr(zeta), loads, n_loads, constants, n_constants,
+                                     program, n_instr, parts, h + N, h, stage_ext)) return rc;
     if (t_evaluations) {
-        if (int rc = evaluate_h_finish(c, ss.st, h, scratch, ext_k, zeta, t_evaluations, t_period, ext_omega_inv, ext_ifft_divisor)) return rc;
+        if (int rc = evaluate_h_finish(c, ss.st, h, h + N, ext_k, zeta, t_evaluations, t_period, ext_omega_inv, ext_ifft_divisor)) return rc;
     }
     return d2h_one(c, out, h, sizeof(Fr) * N, ss.st);
 }
@@ -1474,8 +1425,8 @@ int b200_evaluate_h_dev(const void* const* d_polys, const size_t* lengths, size_
     StreamScope ss(c, stream);
     if (c->stage_c.ensure(sizeof(Fr) * n * (n_coeff ? n_coeff : 1)) || c->stage_b.ensure(sizeof(Fr) * N)) return -2;
     Fr* h = reinterpret_cast<Fr*>(d_out);
-    if (int rc = evaluate_h_parts_on(c, ss.st, reinterpret_cast<const Fr* const*>(d_polys), lengths, n_columns, k, ext_k, as_fr(ext_omega), as_fr(zeta), loads, n_loads,
-                                     constants, n_constants, program, n_instr, c->stage_c.as<Fr>(), c->stage_b.as<Fr>(), h, nullptr)) return rc;
+    if (int rc = evaluate_h_parts_on(c, ss.st, reinterpret_cast<const Fr* const*>(d_polys), lengths, n_columns, k, ext_k, ext_k - k, as_fr(ext_omega), as_fr(zeta),
+                                     loads, n_loads, constants, n_constants, program, n_instr, c->stage_c.as<Fr>(), c->stage_b.as<Fr>(), h, nullptr)) return rc;
     if (!t_evaluations) return 0;
     return evaluate_h_finish(c, ss.st, h, c->stage_b.as<Fr>(), ext_k, zeta, t_evaluations, t_period, ext_omega_inv, ext_ifft_divisor);
 }

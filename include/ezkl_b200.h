@@ -208,7 +208,8 @@ int b200_quotient_eval_dev(const void* const* d_columns, size_t n_columns, uint3
  * the extended domain, or, when t_evaluations != NULL, extended_to_coeff(numerator * t_evaluations[i mod t_period]): the quotient's
  * 2^ext_k coefficients.  A coefficient column crosses PCIe once (its n elements) instead of its coset twice.
  * Device memory: when n_columns * 2^ext_k * 32 B fits the per-call scratch budget (B200_WS_BUDGET_MB, else derived from
- * B200_WS_TOTAL_MB, as for every host-pointer entry point) all columns' cosets are resident at once.  Otherwise (and k >= 1) the
+ * B200_WS_TOTAL_MB, as for every host-pointer entry point) all columns' cosets are resident at once, which holds
+ * n_columns * 2^ext_k * 32 B + (sum of the coefficient columns' lengths) * 32 B + 2 * 2^ext_k * 32 B.  Otherwise (and k >= 1) the
  * numerator is evaluated one n-point coset part at a time (the extended indices c + d i, d = 2^(ext_k - k), for c < d), which holds
  * about n_columns * n * 32 B + (sum of the coefficient columns' lengths) * 32 B + 2 * 2^ext_k * 32 B.  The result is the same bytes
  * either way. */
