@@ -363,6 +363,22 @@ int b200_debug_msm_recode_plan(size_t n, int batch, uint32_t nbuckets, int W, in
     out[0] = p.tile; out[1] = p.tiles;
     return 0;
 }
+// host-only: the launch geometry and workspace of msm_run (msm_plan, msm.cuh) for `batch` columns of n scalars against a table of window
+// c with s windows per level, on a device of sm_count SMs, with the reduction overrides reduce_m / reduce_threads (0: automatic).
+// out = {cap, chunk_stride, heavy_stride, reduce_m, reduce_threads, nparts, final_threads, recode tile, recode tiles, bytes of counts,
+// tile_counts, offs, ents, subs and sums, msm_workspace_per_column}.  -1 for a shape msm_run rejects.
+int b200_debug_msm_plan(size_t n, int batch, int c, int s, int sm_count, int reduce_m, int reduce_threads, uint64_t* out /* 16 */) {
+    if (c < 4 || c > 24) return -1;
+    const int W = (255 + c - 1) / c;
+    if (n == 0 || batch < 1 || s < 1 || s > W || (size_t)batch * s > 65535 || n * W >= ((size_t)1 << 32) || sm_count < 1) return -1;
+    const MsmPlan p = msm_plan(n, batch, c, s, W, sm_count, reduce_m, reduce_threads);
+    MsmTable t;
+    t.n = n; t.c = c; t.W = W; t.s = s; t.L = (W + s - 1) / s;
+    const uint64_t v[16] = {p.cap, p.chunk_stride, p.heavy_stride, p.reduce_m, p.reduce_threads, p.nparts, p.final_threads, p.recode.tile, p.recode.tiles,
+                            p.counts_bytes, p.tile_counts_bytes, p.offs_bytes, p.ents_bytes, p.subs_bytes, p.sums_bytes, msm_workspace_per_column(t, n)};
+    memcpy(out, v, sizeof v);
+    return 0;
+}
 // msm_run with base_off > 0 (the base-split MSM that only a multi-device call makes in the product) on the current device.
 // scalars [batch][n] and bases [table_n] are HOST arrays; out[b] = sum_i scalars[b][i] * bases[base_off + i] in affine form.
 // The table is built with window c under max_table_bytes (0: every level).  The MSM code is msm.cu, linked into this library.

@@ -27,6 +27,8 @@ int b200_debug_digits_host(const b200_fr* s_canonical, size_t n, int c, int32_t*
 int b200_debug_digit_slots_host(const b200_fr* s_canonical, size_t n, int c, int wpl, int32_t* out);
 int b200_debug_msm_pick_levels(size_t n, int c, size_t max_table_bytes, int* s, int* L);
 int b200_debug_msm_recode_plan(size_t n, int batch, uint32_t nbuckets, int W, int sm_count, uint32_t* out);
+/* msm_run's launch geometry and workspace bytes (16 values, see debug.cu); reduce_m / reduce_threads: the tuning overrides, 0 = automatic */
+int b200_debug_msm_plan(size_t n, int batch, int c, int s, int sm_count, int reduce_m, int reduce_threads, uint64_t* out);
 int b200_debug_ntt_plan_host(uint32_t log_n, int batch, int sm_count, int64_t* out);
 int b200_debug_host_g1_op(int op, const b200_g1_affine* a, const b200_g1_affine* b, b200_g1_affine* out, size_t n);
 int b200_debug_host_g1_xyzz_op(int op, const b200_g1_xyzz* a, const b200_g1_xyzz* b, const uint32_t* k, b200_g1_xyzz* out, size_t n);   /* ops 0-4 */

@@ -24,10 +24,6 @@
 
 namespace b200 {
 
-static constexpr int HEAVY_CHUNKS = 32;     // buckets with more chunks than this are summed by a whole block
-static constexpr int REDUCE_M_MAX = 32;      // buckets per thread in k_reduce for large (work-bound) batches; small batches take fewer (latency)
-static constexpr int TREE_THREADS = 256;
-
 int msm_default_window(size_t n) {
     int k = 0;
     while (((size_t)1 << (k + 1)) <= n) ++k;
@@ -199,7 +195,7 @@ __global__ void __launch_bounds__(1024) k_scan_buckets(const uint32_t* __restric
     if (threadIdx.x == 0) sh_max = 0;
     __syncthreads();
     const uint32_t col = blockIdx.x;
-    const uint32_t lc = 31u - (uint32_t)__clz(cap);            // cap is a power of two (pick_cap)
+    const uint32_t lc = 31u - (uint32_t)__clz(cap);            // cap is a power of two (msm_pick_cap)
     const uint32_t* cnt = counts + (size_t)col * nbuckets;
     uint32_t* off = offs + (size_t)col * (nbuckets + 1);
     uint32_t* coff = chunk_offs + (size_t)col * (nbuckets + 1);
@@ -532,14 +528,6 @@ int g1_sum_run(const G1Xyzz* d_points, size_t groups, size_t count, G1Xyzz* d_ou
 }
 
 // ---------------------------------------------------------------------------------------------------------
-static uint32_t pick_cap(size_t total_entries) {
-    // aim for >= ~4 chunks per resident thread slot (SMs x 512 threads), chunk length a power of two in [16, 512]
-    size_t target = total_entries / ((size_t)sm_count() * 512 * 4);
-    uint32_t cap = 16;
-    while (cap < 512 && cap < target) cap <<= 1;
-    return cap;
-}
-
 size_t msm_workspace_per_column(const MsmTable& t, size_t n) {
     const size_t nb = (size_t)t.s << (t.c - 1), ents = n * t.W;      // s bucket sets per column
     const size_t chunk_stride = nb + ents / 16 + 1;
@@ -562,48 +550,29 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     const int vcols = batch * s;
     const size_t ent_stride = (size_t)n * W;
     B200_CHECK(ent_stride < ((size_t)1 << 32), -1, "msm: n*W too large");
-    const Config& cfg = config();
-    const uint32_t cap = pick_cap(ent_stride * batch);
-    const size_t chunk_stride = (size_t)nb + ent_stride / cap + 1;
-    const uint32_t heavy_stride = (uint32_t)(ent_stride / ((size_t)cap * HEAVY_CHUNKS)) + 2;
-    // Bucket reduction geometry.  A thread owns reduce_m consecutive buckets (2 * reduce_m dependent additions, then a small-multiple
-    // fix-up and a block tree).  Large batches are work bound: 32 buckets per thread, 256-thread CTAs.  Small batches are bound by the
-    // LATENCY of that dependent chain (a lone warp needs ~7.5 us per group addition, about 1000 cycles per field multiplication, twice its
-    // throughput cost), so fewer buckets per thread and more, smaller CTAs win until the extra threads' fix-ups and tree levels cost more
-    // than the shorter chain saves.  The table is the optimum per total bucket count of the sweep in tools/bench_msm_tail_sweep.py.
-    const size_t all_buckets = (size_t)batch * nb;
-    uint32_t reduce_m = REDUCE_M_MAX, reduce_threads = TREE_THREADS;
-    if (all_buckets <= ((size_t)1 << 15)) { reduce_m = 4; reduce_threads = 128; }
-    else if (all_buckets <= ((size_t)1 << 18)) { reduce_m = 8; reduce_threads = 128; }
-    else if (all_buckets <= ((size_t)5 << 17)) { reduce_m = 16; reduce_threads = 256; }
-    else if (all_buckets < ((size_t)37 << 15)) { reduce_m = 32; reduce_threads = 128; }
-    while (reduce_m > 1 && reduce_m > half) reduce_m >>= 1;
-    if (cfg.msm_reduce_m >= 1 && cfg.msm_reduce_m <= 4096) reduce_m = (uint32_t)cfg.msm_reduce_m;    // tuning override
-    if (cfg.msm_reduce_threads == 32 || cfg.msm_reduce_threads == 64 || cfg.msm_reduce_threads == 128 || cfg.msm_reduce_threads == 256) reduce_threads = (uint32_t)cfg.msm_reduce_threads;
-    const uint32_t nparts = div_up(div_up(half, reduce_m), reduce_threads);
-    uint32_t final_threads = 32;
-    while (final_threads < (uint32_t)TREE_THREADS && final_threads < nparts) final_threads <<= 1;
-
     const unsigned sms = (unsigned)sm_count();
-    const MsmRecodePlan rp = msm_pick_recode(n, batch, nb, W, (int)sms);
+    const MsmPlan plan = msm_plan(n, batch, c, s, W, (int)sms, config().msm_reduce_m, config().msm_reduce_threads);
+    const uint32_t cap = plan.cap, heavy_stride = plan.heavy_stride, reduce_m = plan.reduce_m, reduce_threads = plan.reduce_threads;
+    const uint32_t nparts = plan.nparts, final_threads = plan.final_threads;
+    const size_t chunk_stride = plan.chunk_stride;
+    const MsmRecodePlan rp = plan.recode;
     // counts region: hist | cursor | len_hist | len_cursor | heavy, zeroed every call (hist first: k_scan_buckets reads it as uint4).
     // The shared-counter path writes every hist word (k_tile_prefix) and has no cursor, so it zeroes from len_hist on.
-    const size_t n_hist = (size_t)batch * nb, n_len = (size_t)batch * (cap + 1), n_heavy = (size_t)batch * heavy_stride;
-    const size_t counts_words = 2 * n_hist + 2 * n_len + n_heavy;
-    if (ws.counts.ensure(counts_words * 4)) return -2;
+    const size_t n_hist = (size_t)batch * nb, n_len = (size_t)batch * (cap + 1);
+    if (ws.counts.ensure(plan.counts_bytes)) return -2;
     uint32_t* hist = ws.counts.as<uint32_t>();
     uint32_t* cursor = hist + n_hist;
     uint32_t* len_hist = cursor + n_hist;
     uint32_t* len_cursor = len_hist + n_len;
     uint32_t* heavy = len_cursor + n_len;
     uint32_t* zero_from = rp.tile ? len_hist : hist;
-    const size_t zero_words = counts_words - (size_t)(zero_from - hist);
+    const size_t zero_words = plan.counts_bytes / 4 - (size_t)(zero_from - hist);
     uint32_t* tile_counts = nullptr;
     const size_t tile_smem = (size_t)nb * 4;
     auto* count_k = s == 1 ? k_digits_tile<false, false> : k_digits_tile<false, true>;
     auto* place_k = s == 1 ? k_digits_tile<true, false> : k_digits_tile<true, true>;
     if (rp.tile) {
-        if (ws.tile_counts.ensure((size_t)batch * rp.tiles * nb * 4)) return -2;
+        if (ws.tile_counts.ensure(plan.tile_counts_bytes)) return -2;
         tile_counts = ws.tile_counts.as<uint32_t>();
         // the attribute belongs to the function on this device, not to the call: always the same limit, so concurrent callers with
         // other bucket counts cannot lower it under each other's launches (each launch still reserves only nb * 4 bytes)
@@ -613,20 +582,19 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
     }
     // offsets: offs | chunk_offs | len_offs
     const size_t n_off = (size_t)batch * (nb + 1);
-    if (ws.offs.ensure((2 * n_off + n_len + (size_t)batch) * 4)) return -2;
+    if (ws.offs.ensure(plan.offs_bytes)) return -2;
     uint32_t* offs = ws.offs.as<uint32_t>();
     uint32_t* chunk_offs = offs + n_off;
     uint32_t* len_offs = chunk_offs + n_off;
     uint32_t* skew = len_offs + n_len;
-    if (ws.ents.ensure((size_t)batch * ent_stride * 4)) return -2;
+    if (ws.ents.ensure(plan.ents_bytes)) return -2;
     uint32_t* ents = ws.ents.as<uint32_t>();
-    if (ws.subs.ensure((size_t)batch * chunk_stride * 4 * 3)) return -2;
+    if (ws.subs.ensure(plan.subs_bytes)) return -2;
     uint32_t* chunk_start = ws.subs.as<uint32_t>();
     uint32_t* chunk_len = chunk_start + (size_t)batch * chunk_stride;
     uint32_t* order = chunk_len + (size_t)batch * chunk_stride;
     // sums: chunk_sums | bucket_sums | partials | set_sums (s > 1: one result per bucket set, folded by k_subwindow_fold)
-    const size_t n_set = s > 1 ? (size_t)vcols : 0;
-    if (ws.sums.ensure(sizeof(G1Xyzz) * ((size_t)batch * chunk_stride + (size_t)batch * nb + (size_t)vcols * nparts + n_set))) return -2;
+    if (ws.sums.ensure(plan.sums_bytes)) return -2;
     G1Xyzz* chunk_sums = ws.sums.as<G1Xyzz>();
     G1Xyzz* bucket_sums = chunk_sums + (size_t)batch * chunk_stride;
     G1Xyzz* partials = bucket_sums + (size_t)batch * nb;

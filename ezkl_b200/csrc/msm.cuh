@@ -68,6 +68,68 @@ inline MsmRecodePlan msm_pick_recode(size_t n, int batch, uint32_t nb, int W, in
     p.tiles = (uint32_t)((n + tile - 1) / tile);
     return p;
 }
+static constexpr int HEAVY_CHUNKS = 32;     // buckets with more chunks than this are summed by a whole block (k_combine_heavy)
+static constexpr int REDUCE_M_MAX = 32;     // buckets per thread in k_reduce for large (work-bound) batches; small batches take fewer (latency)
+static constexpr int TREE_THREADS = 256;
+
+// Chunk length cap: aim for >= ~4 chunks per resident thread slot (SMs x 512 threads), a power of two in [16, 512].
+inline uint32_t msm_pick_cap(size_t total_entries, int sms) {
+    const size_t target = total_entries / ((size_t)sms * 512 * 4);
+    uint32_t cap = 16;
+    while (cap < 512 && cap < target) cap <<= 1;
+    return cap;
+}
+
+// Launch geometry and workspace of one msm_run call: `batch` columns of n scalars against a table of window c, W windows and s
+// bucket sets per column, on a device of `sms` SMs.  reduce_m / reduce_threads are the B200_MSM_REDUCE_M / _THREADS overrides
+// (0 or out of range: the automatic choice).  Pure host function; msm_run launches exactly this.
+struct MsmPlan {
+    uint32_t cap = 0;               // entries per chunk at most (k_scan_buckets, k_fill_chunks)
+    size_t chunk_stride = 0;        // chunk slots per column: >= the chunks any histogram of n * W entries can make
+    uint32_t heavy_stride = 0;      // heavy-list words per column: a count, then room for every bucket of > HEAVY_CHUNKS chunks
+    uint32_t reduce_m = 0, reduce_threads = 0;     // k_reduce: buckets per thread, threads per CTA
+    uint32_t nparts = 0;            // k_reduce CTAs per bucket set, i.e. partials per bucket set that k_final adds
+    uint32_t final_threads = 0;     // k_final threads per CTA
+    MsmRecodePlan recode;
+    // bytes each MsmWorkspace buffer is asked for
+    size_t counts_bytes = 0, tile_counts_bytes = 0, offs_bytes = 0, ents_bytes = 0, subs_bytes = 0, sums_bytes = 0;
+};
+inline MsmPlan msm_plan(size_t n, int batch, int c, int s, int W, int sms, int reduce_m, int reduce_threads) {
+    MsmPlan p;
+    const uint32_t half = 1u << (c - 1), nb = half * (uint32_t)s;
+    const size_t vcols = (size_t)batch * s, ent_stride = n * (size_t)W;
+    p.cap = msm_pick_cap(ent_stride * batch, sms);
+    p.chunk_stride = (size_t)nb + ent_stride / p.cap + 1;
+    p.heavy_stride = (uint32_t)(ent_stride / ((size_t)p.cap * HEAVY_CHUNKS)) + 2;
+    // Bucket reduction geometry.  A thread owns reduce_m consecutive buckets (2 * reduce_m dependent additions, then a small-multiple
+    // fix-up and a block tree).  Large batches are work bound: 32 buckets per thread, 256-thread CTAs.  Small batches are bound by the
+    // LATENCY of that dependent chain (a lone warp needs ~7.5 us per group addition, about 1000 cycles per field multiplication, twice its
+    // throughput cost), so fewer buckets per thread and more, smaller CTAs win until the extra threads' fix-ups and tree levels cost more
+    // than the shorter chain saves.  The table is the optimum per total bucket count of the sweep in tools/bench_msm_tail_sweep.py.
+    const size_t all_buckets = (size_t)batch * nb;
+    p.reduce_m = REDUCE_M_MAX; p.reduce_threads = TREE_THREADS;
+    if (all_buckets <= ((size_t)1 << 15)) { p.reduce_m = 4; p.reduce_threads = 128; }
+    else if (all_buckets <= ((size_t)1 << 18)) { p.reduce_m = 8; p.reduce_threads = 128; }
+    else if (all_buckets <= ((size_t)5 << 17)) { p.reduce_m = 16; p.reduce_threads = 256; }
+    else if (all_buckets < ((size_t)37 << 15)) { p.reduce_m = 32; p.reduce_threads = 128; }
+    while (p.reduce_m > 1 && p.reduce_m > half) p.reduce_m >>= 1;
+    if (reduce_m >= 1 && reduce_m <= 4096) p.reduce_m = (uint32_t)reduce_m;    // tuning override
+    if (reduce_threads == 32 || reduce_threads == 64 || reduce_threads == 128 || reduce_threads == 256) p.reduce_threads = (uint32_t)reduce_threads;
+    p.nparts = (((half + p.reduce_m - 1) / p.reduce_m) + p.reduce_threads - 1) / p.reduce_threads;
+    p.final_threads = 32;
+    while (p.final_threads < (uint32_t)TREE_THREADS && p.final_threads < p.nparts) p.final_threads <<= 1;
+    p.recode = msm_pick_recode(n, batch, nb, W, sms);
+    // counts: hist | cursor | len_hist | len_cursor | heavy;  offs: offs | chunk_offs | len_offs | skew;  subs: chunk start | length | order;
+    // sums: chunk_sums | bucket_sums | partials | set_sums (s > 1)
+    const size_t n_hist = (size_t)batch * nb, n_len = (size_t)batch * (p.cap + 1), n_off = (size_t)batch * (nb + 1);
+    p.counts_bytes = (2 * n_hist + 2 * n_len + (size_t)batch * p.heavy_stride) * 4;
+    p.tile_counts_bytes = p.recode.tile ? (size_t)batch * p.recode.tiles * nb * 4 : 0;
+    p.offs_bytes = (2 * n_off + n_len + (size_t)batch) * 4;
+    p.ents_bytes = (size_t)batch * ent_stride * 4;
+    p.subs_bytes = (size_t)batch * p.chunk_stride * 4 * 3;
+    p.sums_bytes = sizeof(G1Xyzz) * ((size_t)batch * p.chunk_stride + n_hist + vcols * p.nparts + (s > 1 ? vcols : 0));
+    return p;
+}
 // Picks the window (c <= 0: msm_default_window) and the level count, and allocates the table.  Level 0 (the first n points)
 // is left for the caller to fill, e.g. by uploading the bases straight into it.
 int msm_table_alloc(MsmTable* t, size_t n, int c, size_t max_table_bytes);

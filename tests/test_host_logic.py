@@ -27,11 +27,11 @@ def test_cabi_exports_every_declared_symbol():
             assert fn.argtypes == argtypes and fn.restype is restype, name
 
 
-def test_cabi_signatures_and_counts_follow_the_headers():
+def test_cabi_signatures_and_hook_counts_follow_the_headers():
     """Pointers are c_void_p; int, uint32_t, uint64_t and size_t keep their C width; every declared function is typed.  The
-    headers declare 66 product entry points and 17 test hooks."""
+    headers declare 66 product entry points and 18 test hooks."""
     prod, dbg = nat.declarations(nat.HEADER), nat.declarations(nat.DBG_HEADER)
-    assert (len(prod), len(dbg)) == (66, 17)
+    assert (len(prod), len(dbg)) == (66, 18)
     for decls in (prod, dbg):
         for name, (argtypes, restype) in decls.items():
             assert set(argtypes) <= {C.c_void_p, C.c_int, C.c_uint32, C.c_uint64, C.c_size_t}, name
@@ -44,6 +44,7 @@ def test_cabi_signatures_and_counts_follow_the_headers():
                                      C.c_int, C.c_void_p, C.c_size_t, C.c_void_p], C.c_int)
     assert dbg["b200_debug_msm_pick_levels"] == ([C.c_size_t, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p], C.c_int)
     assert dbg["b200_debug_ntt_plan_host"] == ([C.c_uint32, C.c_int, C.c_int, C.c_void_p], C.c_int)
+    assert dbg["b200_debug_msm_plan"] == ([C.c_size_t] + [C.c_int] * 6 + [C.c_void_p], C.c_int)
     assert dbg["b200_debug_g1_xyzz_op"] == dbg["b200_debug_host_g1_xyzz_op"] == ([C.c_int] + [C.c_void_p] * 4 + [C.c_size_t], C.c_int)
     assert dbg["b200_debug_field_op4"] == dbg["b200_debug_host_field_op4"] == ([C.c_int, C.c_int] + [C.c_void_p] * 5 + [C.c_size_t], C.c_int)
 
