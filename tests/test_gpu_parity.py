@@ -335,31 +335,21 @@ def test_cpp_host_mirror():
     assert r.returncode == 0 and r.stdout.strip().endswith("OK"), r.stdout + r.stderr
 
 
-def test_sharding_layer_single_rank_device_paths():
-    """world = 1 degenerate run of the multi-GPU layer on one GPU: the device implementations behind ShardedMsm /
-    ShardedNtt (msm_batch -> g1_sum -> normalize; transposed batched NTTs + twiddle matrix) against the oracle."""
+def test_msm_base_slice_partials_sum_to_oracle():
+    """An MSM split by hand into 4 base slices: msm_batch on each slice, g1_sum of the XYZZ partials, normalize — the
+    same point the oracle's whole MSM gives, for both columns of the batch."""
     import torch
     from ezkl_b200 import device as dev
-    from ezkl_b200 import parallel as par
     n = 1 << 12
     bases_np = orc.gen_bases(n, seed=31)
     sc = np.stack([orc.gen_scalars(n, seed=32), orc.gen_scalars(n, seed=33)])
-    sm = par.ShardedMsm(dev.from_host(bases_np), n)
-    got = sm(dev.from_host(sc))
-    for i in range(2):
-        assert np.array_equal(jac_to_affine(got[i])[0], orc.msm(sc[i], bases_np, THREADS))
-    # g1_sum of several partials: split the MSM in 4 slices by hand and add
     parts = []
     for lo in range(0, n, n // 4):
         b = dev.DeviceBases(dev.from_host(bases_np[lo:lo + n // 4]))
         parts.append(dev.msm_batch(b, dev.from_host(sc[:, lo:lo + n // 4])))
-    summed = dev.g1_sum(torch.stack(parts, dim=1).contiguous())
-    assert np.array_equal(dev.normalize(summed), got)
-    for k in (9, 14):
-        a = orc.gen_scalars(1 << k, seed=k)
-        s = par.ShardedNtt(k, pyref.omega_for(k))
-        out = s.gather(s.forward(s.scatter(dev.from_host(a))))
-        assert np.array_equal(dev.to_host(out), orc.best_fft(a, k, orc.omega(k), THREADS))
+    got = dev.normalize(dev.g1_sum(torch.stack(parts, dim=1).contiguous()))
+    for i in range(2):
+        assert np.array_equal(jac_to_affine(got[i])[0], orc.msm(sc[i], bases_np, THREADS))
 
 
 def test_reentrancy_from_threads():

@@ -1,5 +1,5 @@
-"""World-size-2 gloo test (CPU) of the sharding layer's host logic: the round-robin column deal, contiguous pair slices,
-the padded all-gather of per-rank results and its inverse interleave — the plumbing bench.py --gpus N and ShardedMsm use."""
+"""World-size-2 gloo test (CPU) of the column-dealing layer's host logic: the round-robin column deal, the padded all-gather
+of per-rank results and its inverse interleave — the plumbing bench.py --gpus N uses."""
 import os
 import socket
 
@@ -31,10 +31,6 @@ def _worker(rank, world, port, total):
     assert full.shape == (total, 16)
     for c in range(total):
         assert int(full[c, 0]) == c * 1000 and int(full[c, 15]) == c * 1000 + 15
-    # contiguous pair slices tile [0, n) exactly
-    n = 1000003
-    bounds = [par.slice_bounds(n, q, world) for q in range(world)]
-    assert bounds[0][0] == 0 and bounds[-1][1] == n and all(bounds[i][1] == bounds[i + 1][0] for i in range(world - 1))
     dist.barrier()
     dist.destroy_process_group()
 
@@ -44,77 +40,5 @@ def test_column_deal_allgather_world2():
     mp.spawn(_worker, args=(2, port, 7), nprocs=2, join=True)
 
 
-def test_slice_bounds_and_owner():
-    for n in (1, 5, 64, 1000):
-        for world in (1, 2, 4, 8):
-            tot = 0
-            for r in range(world):
-                lo, hi = par.slice_bounds(n, r, world)
-                assert hi >= lo
-                tot += hi - lo
-            assert tot == n
+def test_column_owner():
     assert [par.column_owner(i, 4) for i in range(6)] == [0, 1, 2, 3, 0, 1]
-
-
-# ---- six-step NTT index logic on CPU (gloo), with the bigint restatement as the local transform -------------------------
-def _sixstep_worker(rank, world, port, k):
-    import numpy as np
-    from oracle import pyref
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
-    par.init_distributed("gloo")
-    R = pyref.R
-    n = 1 << k
-    w = pyref.omega_for(k)
-    rng = __import__("random").Random(5)
-    xs = [rng.randrange(1 << 60) for _ in range(n)]          # small values so int64 tensors can carry them through gloo
-
-    # stand-ins on CPU int64 tensors (values < 2^61 are reduced mod a 61-bit prime field instead of Fr: the index logic is
-    # field-agnostic).  Use a small NTT-friendly prime: p = 2^32 * 3 + 1 = 12884901889? keep it simple: p = 257-like is too
-    # small, so use p = 998244353 (2^23 * 7 * 17 + 1, generator 3).
-    P = 998244353
-    gen = 3
-    wk = pow(gen, (P - 1) >> k, P)
-    xs = [x % P for x in xs]
-
-    def dft(a, root):
-        m = len(a)
-        return [sum(a[i] * pow(root, i * j, P) for i in range(m)) % P for j in range(m)]
-
-    def local_ntt(rows, log_m, root):
-        out = torch.empty_like(rows)
-        for b in range(rows.shape[0]):
-            out[b, :, 0] = torch.tensor(dft([int(v) for v in rows[b, :, 0]], root), dtype=torch.int64)
-        return out
-
-    def mul(a, b):
-        return (a * b) % P
-
-    class S(par.ShardedNtt):
-        pass
-
-    def make_tw():
-        c2, N1 = (1 << (k - (k + 1) // 2)) // world, 1 << ((k + 1) // 2)
-        t = torch.empty((c2, N1, 1), dtype=torch.int64)
-        for i2l in range(c2):
-            i2 = rank * c2 + i2l
-            for j1 in range(N1):
-                t[i2l, j1, 0] = pow(wk, j1 * i2, P)
-        return t
-
-    import ezkl_b200.fields as F
-    saved = F.FR_MODULUS
-    F.FR_MODULUS = P                      # the class derives omega^(N2), omega^(N1) with this modulus
-    try:
-        s = S(k, wk, local_ntt=local_ntt, mul=mul, make_twiddles=make_tw)
-        full = torch.tensor(xs, dtype=torch.int64).reshape(n, 1)
-        out = s.gather(s.forward(s.scatter(full)))
-    finally:
-        F.FR_MODULUS = saved
-    assert [int(v) for v in out[:, 0]] == dft(xs, wk)
-    dist.barrier()
-    dist.destroy_process_group()
-
-
-def test_sixstep_ntt_layout_world2():
-    port = _free_port()
-    mp.spawn(_sixstep_worker, args=(2, port, 6), nprocs=2, join=True)
