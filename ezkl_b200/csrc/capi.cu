@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "../../include/ezkl_b200.h"
+#include "../../include/ezkl_b200_keygen.h"
 #include "../../include/ezkl_b200_resident.h"
 #include "msm.cuh"
 #include "ntt.cuh"
@@ -364,6 +365,19 @@ static NttPlan* warm_plan(int slot, uint32_t log_n, const Fr& omega, cudaStream_
     NttPlan* p = nc.get(log_n, omega, st);
     if (p && nc.plans.size() != before) cudaStreamSynchronize(st);   // tables complete before other threads use them
     return p;
+}
+
+// the two-level power table that k_poly_coset_fold and k_perm_sigmas read: tab = [w^e, e < 2^lo_bits | w^(e << lo_bits), e < 2^(log_n - lo_bits)],
+// so that w^e = tab[e mod 2^lo_bits] * tab[2^lo_bits + (e >> lo_bits)] for every e < 2^log_n
+static void omega_power_table(Fr* tab, uint32_t lo_bits, uint32_t log_n, const Fr& w) {
+    const size_t n_lo = (size_t)1 << lo_bits, n_hi = (size_t)1 << (log_n - lo_bits);
+    Fr* lo = tab;
+    Fr* hi = tab + n_lo;
+    lo[0] = fp_one<FrTag>();
+    for (size_t e = 1; e < n_lo; ++e) lo[e] = lo[e - 1] * w;
+    const Fr step = lo[n_lo - 1] * w;
+    hi[0] = fp_one<FrTag>();
+    for (size_t e = 1; e < n_hi; ++e) hi[e] = hi[e - 1] * step;
 }
 
 // ---- internal call layer: <op>_on(c, st, ...) validates the device-side arguments, converts host constants and runs the
@@ -1224,6 +1238,111 @@ int b200_lookup_multiplicities(const b200_fr* table, size_t n_table, const b200_
     return 0;
 }
 
+// ---- permutation keygen (include/ezkl_b200_keygen.h) ------------------------------------------------------------------------
+// n_map_columns mapping columns at d_map -> sigma columns at d_out (stride out_stride); a cell is valid when its column is < n_columns and its
+// row < 2^k.  The host-pointer entry point calls this once per column group, with n_columns = every column of the key.
+static int perm_sigmas_on(Ctx* c, cudaStream_t st, const void* d_map, size_t n_map_columns, size_t n_columns, uint32_t k, const b200_fr* omega, const b200_fr* delta,
+                          void* d_out, size_t out_stride, unsigned long long* d_invalid) {
+    B200_CHECK(d_map && d_out && omega && delta, -1, "permutation_sigmas: null pointer");
+    B200_CHECK(n_columns < (1ull << 32), -1, "permutation_sigmas: %zu columns, at most 2^32 - 1", n_columns);
+    const uint32_t lo_bits = (k + 1) / 2;
+    std::vector<Fr> tab(n_columns + ((size_t)1 << lo_bits) + ((size_t)1 << (k - lo_bits)));
+    const Fr d = as_fr(delta);
+    tab[0] = fp_one<FrTag>();
+    for (size_t j = 1; j < n_columns; ++j) tab[j] = tab[j - 1] * d;
+    omega_power_table(tab.data() + n_columns, lo_bits, k, as_fr(omega));
+    return perm_sigmas_run(reinterpret_cast<const uint32_t*>(d_map), n_map_columns, k, tab.data(), n_columns, lo_bits, reinterpret_cast<Fr*>(d_out), out_stride, d_invalid,
+                           c->ring, st);
+}
+int b200_permutation_sigmas_dev(const void* d_mapping, size_t n_columns, uint32_t k, const b200_fr* omega, const b200_fr* delta, void* d_out, size_t out_stride,
+                                uint64_t* invalid, void* stream) {
+    B200_ENTER(c, d_out);
+    B200_CHECK(k <= 28, -1, "permutation_sigmas_dev: k = %u out of range [0, 28]", k);
+    B200_CHECK(out_stride >= ((size_t)1 << k), -1, "permutation_sigmas_dev: out_stride %zu < 2^%u", out_stride, k);
+    if (n_columns == 0) return 0;
+    B200_CHECK(d_mapping && d_out && omega && delta, -1, "permutation_sigmas_dev: null pointer");
+    StreamScope ss(c, stream);
+    unsigned long long* d_inv = nullptr;
+    if (invalid) {
+        if (c->small.ensure(sizeof(unsigned long long))) return -2;
+        d_inv = c->small.as<unsigned long long>();
+        B200_CUDA(cudaMemsetAsync(d_inv, 0, sizeof *d_inv, ss.st));
+    }
+    if (int rc = perm_sigmas_on(c, ss.st, d_mapping, n_columns, n_columns, k, omega, delta, d_out, out_stride, d_inv)) return rc;
+    if (invalid) {
+        unsigned long long h = 0;
+        B200_CUDA(cudaMemcpyAsync(&h, d_inv, sizeof h, cudaMemcpyDeviceToHost, ss.st));
+        B200_CUDA(cudaStreamSynchronize(ss.st));
+        *invalid = h;
+    }
+    return 0;
+}
+// index of the first cell (column >= n_columns or row >= n) of the host mapping, or `cells` when every cell is valid; large mappings are
+// scanned by several host threads
+static size_t first_invalid_cell(const uint32_t* map, size_t cells, size_t n_columns, size_t n) {
+    auto scan = [=](size_t lo, size_t hi) { for (size_t e = lo; e < hi; ++e) if (map[2 * e] >= n_columns || map[2 * e + 1] >= n) return e; return cells; };
+    const size_t T = cells >= ((size_t)1 << 22) ? 8 : 1, part = (cells + T - 1) / T;
+    std::vector<size_t> first(T, cells);
+    std::vector<std::thread> th;
+    for (size_t t = 1; t < T; ++t) th.emplace_back([&, t] { first[t] = scan(t * part < cells ? t * part : cells, (t + 1) * part < cells ? (t + 1) * part : cells); });
+    first[0] = scan(0, part < cells ? part : cells);
+    for (auto& x : th) x.join();
+    for (size_t t = 0; t < T; ++t) if (first[t] < cells) return first[t];
+    return cells;
+}
+// host path on ONE device: the columns cols[0 .. count) of the mapping -> out[cols[.]], staged in column groups bounded by the call budget
+static int perm_sigmas_host_on(Ctx* c, const uint32_t* mapping, const size_t* cols, size_t count, size_t n_columns, uint32_t k, const b200_fr* omega,
+                               const b200_fr* delta, b200_fr* const* out) {
+    if (count == 0) return 0;
+    DevGuard dg(c);
+    const size_t n = (size_t)1 << k, map_bytes = 2 * sizeof(uint32_t) * n, col_bytes = sizeof(Fr) * n;
+    size_t sub = call_budget() / (map_bytes + col_bytes);
+    if (sub < 1) sub = 1;
+    if (sub > count) sub = count;
+    if (c->stage_a.ensure(map_bytes * sub) || c->stage_b.ensure(col_bytes * sub)) return -2;
+    StreamScope ss(c, nullptr);
+    for (size_t b0 = 0; b0 < count; b0 += sub) {
+        const size_t nb = count - b0 < sub ? count - b0 : sub;
+        std::vector<HostSeg> up, down;            // adjacent columns (in the mapping, and in the caller's output) merge into one segment
+        for (size_t b = b0; b < b0 + nb; ++b) {
+            uint8_t* m = (uint8_t*)const_cast<uint32_t*>(mapping + 2 * n * cols[b]);
+            uint8_t* o = (uint8_t*)out[cols[b]];
+            if (!up.empty() && up.back().p + up.back().bytes == m) up.back().bytes += map_bytes; else up.push_back(HostSeg{m, map_bytes});
+            if (!down.empty() && down.back().p + down.back().bytes == o) down.back().bytes += col_bytes; else down.push_back(HostSeg{o, col_bytes});
+        }
+        if (int rc = h2d_segments(c, c->stage_a.p, up.data(), up.size(), ss.st)) return rc;
+        if (int rc = perm_sigmas_on(c, ss.st, c->stage_a.p, nb, n_columns, k, omega, delta, c->stage_b.p, n, nullptr)) return rc;
+        if (int rc = d2h_segments(c, c->stage_b.p, down.data(), down.size(), ss.st)) return rc;
+    }
+    return 0;
+}
+int b200_permutation_sigmas(const uint32_t* mapping, size_t n_columns, uint32_t k, const b200_fr* omega, const b200_fr* delta, b200_fr* const* out) {
+    B200_ENTER(c, nullptr);
+    B200_CHECK(k <= 28, -1, "permutation_sigmas: k = %u out of range [0, 28]", k);
+    if (n_columns == 0) return 0;
+    B200_CHECK(mapping && omega && delta && out, -1, "permutation_sigmas: null pointer");
+    B200_CHECK(n_columns < (1ull << 32), -1, "permutation_sigmas: %zu columns, at most 2^32 - 1", n_columns);
+    for (size_t j = 0; j < n_columns; ++j) B200_CHECK(out[j], -1, "permutation_sigmas: out[%zu] is null", j);
+    const size_t n = (size_t)1 << k, cells = n_columns * n;
+    const size_t bad = first_invalid_cell(mapping, cells, n_columns, n);
+    B200_CHECK(bad == cells, -1, "permutation_sigmas: cell (column %zu, row %zu) maps to (%u, %u), outside %zu columns of 2^%u rows", bad / n, bad % n,
+               mapping[2 * bad], mapping[2 * bad + 1], n_columns, k);
+    const int nd = g_ndev.load();
+    if (nd > 1 && n_columns >= 2 && cells >= ((size_t)1 << 18)) {
+        // column groups dealt round-robin over the devices, as the batched transforms deal polynomials
+        std::lock_guard<std::mutex> lk(g_multi_mu);
+        std::vector<std::vector<size_t>> mine(nd);
+        for (size_t j = 0; j < n_columns; ++j) mine[j % nd].push_back(j);
+        return run_on_slots(nd, [&](int s) -> int {
+            Ctx* cs; if (int r = get_ctx(&cs, s)) return r;
+            return perm_sigmas_host_on(cs, mapping, mine[s].data(), mine[s].size(), n_columns, k, omega, delta, out);
+        });
+    }
+    std::vector<size_t> all(n_columns);
+    for (size_t j = 0; j < n_columns; ++j) all[j] = j;
+    return perm_sigmas_host_on(c, mapping, all.data(), n_columns, n_columns, k, omega, delta, out);
+}
+
 // ---- quotient numerator (evaluate_h) ------------------------------------------------------------------------------
 static_assert(sizeof(b200_instr) == sizeof(QInstr) && sizeof(b200_col_ref) == sizeof(QLoad), "ABI structs must match the kernel's");
 static int quotient_eval_on(Ctx* c, cudaStream_t st, const void* const* d_columns, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_col_ref* loads, size_t n_loads,
@@ -1298,13 +1417,7 @@ static int evaluate_h_parts_on(Ctx* c, cudaStream_t st, const Fr* const* cols, c
         std::vector<uint8_t> blob(tab_bytes + fold_bytes);
         Fr* tab = reinterpret_cast<Fr*>(blob.data());
         tab[0] = fp_one<FrTag>(); tab[1] = zeta; tab[2] = zeta * zeta;
-        Fr* lo = tab + 3;
-        Fr* hi = lo + n_lo;
-        lo[0] = fp_one<FrTag>();
-        for (size_t e = 1; e < n_lo; ++e) lo[e] = lo[e - 1] * ext_omega;
-        const Fr step = lo[n_lo - 1] * ext_omega;
-        hi[0] = fp_one<FrTag>();
-        for (size_t e = 1; e < n_hi; ++e) hi[e] = hi[e - 1] * step;
+        omega_power_table(tab + 3, lo_bits, ext_k, ext_omega);
         memcpy(blob.data() + tab_bytes, fold.data(), fold_bytes);
         if (int rc = ring_upload(c, c->small.p, blob.data(), blob.size(), st)) return rc;
         d_tab = c->small.as<Fr>();

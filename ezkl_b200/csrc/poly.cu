@@ -107,6 +107,38 @@ int poly_coset_fold(const FoldCol* d_cols, size_t n_cols, const Fr* d_tab, uint3
     return 0;
 }
 
+// ---- permutation keygen: sigma columns from the copy-constraint mapping -----------------------------------------------
+// cell e = j * n + i of the mapping holds (column c, row r) of the cell its cycle maps (j, i) to; out[j * out_stride + i] =
+// delta^c * omega^r.  tab = [delta^c, c < n_delta | lo | hi] with omega^r = lo[r mod 2^lo_bits] * hi[r >> lo_bits].  Per cell: 8 B read,
+// 32 B written and two multiplications, so the kernel is HBM-bound; the tables stay in L1 / L2.
+__global__ void __launch_bounds__(256) k_perm_sigmas(const uint2* __restrict__ map, size_t cells, uint32_t k, const Fr* __restrict__ tab, uint32_t n_delta,
+                                                     uint32_t lo_bits, Fr* __restrict__ out, size_t out_stride, unsigned long long* __restrict__ invalid) {
+    const uint32_t n_mask = (uint32_t)(((uint64_t)1 << k) - 1), lo_mask = (1u << lo_bits) - 1;
+    const Fr* lo = tab + n_delta;
+    const Fr* hi = lo + ((size_t)1 << lo_bits);
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < cells; e += (size_t)gridDim.x * blockDim.x) {
+        const uint2 m = map[e];
+        Fr v = fp_zero<FrTag>();
+        if (m.x < n_delta && m.y <= n_mask) v = fp_load(tab + m.x) * (fp_load(lo + (m.y & lo_mask)) * fp_load(hi + (m.y >> lo_bits)));
+        else if (invalid) atomicAdd(invalid, 1ull);
+        fp_store(out + (e >> k) * out_stride + (e & n_mask), v);
+    }
+}
+int perm_sigmas_run(const uint32_t* d_map, size_t n_columns, uint32_t k, const Fr* h_tab, size_t n_delta, uint32_t lo_bits, Fr* d_out, size_t out_stride,
+                    unsigned long long* d_invalid, StagingRing& ring, cudaStream_t st) {
+    B200_CHECK(k <= 28 && lo_bits <= k && n_delta < (1ull << 32) && out_stride >= ((size_t)1 << k), -1, "perm_sigmas: bad argument");
+    if (n_columns == 0) return 0;
+    const size_t tab_elems = n_delta + ((size_t)1 << lo_bits) + ((size_t)1 << (k - lo_bits)), cells = n_columns << k;
+    const void* d_tab;
+    if (int rc = ring.push(h_tab, sizeof(Fr) * tab_elems, st, &d_tab)) return rc;
+    ProfScope ps(PROF_POLY, st);
+    k_perm_sigmas<<<ew_grid(cells), 256, 0, st>>>(reinterpret_cast<const uint2*>(d_map), cells, k, reinterpret_cast<const Fr*>(d_tab), (uint32_t)n_delta, lo_bits,
+                                                  d_out, out_stride, d_invalid);
+    count_launch();
+    B200_CUDA(cudaGetLastError());
+    return 0;
+}
+
 // ---- shared-memory helpers for one Fr per thread -------------------------------------------------------------
 DEV Fr shf_get(const Fr* sh, uint32_t i) { return fp_load(sh + i); }
 DEV void shf_put(Fr* sh, uint32_t i, const Fr& v) { fp_store(sh + i, v); }

@@ -22,6 +22,12 @@ int poly_scale_cycle(const Fr* a, const Fr* h_consts, uint32_t period, Fr* out, 
 struct FoldCol { const Fr* a; uint64_t len; };
 int poly_coset_fold(const FoldCol* d_cols, size_t n_cols, const Fr* d_tab, uint32_t lo_bits, uint32_t log_w, uint64_t mul, Fr* out, size_t out_stride, size_t n,
                     cudaStream_t st);
+// permutation sigma columns (halo2 permutation/keygen.rs build_pk): d_map = n_columns * 2^k (column, row) uint32 pairs, column-major;
+// d_out[j * out_stride + i] = delta^column * omega^row of cell (j, i).  h_tab = [delta^c, c < n_delta | omega^e, e < 2^lo_bits |
+// omega^(e << lo_bits), e < 2^(k - lo_bits)] (host, staged through `ring`).  A cell with column >= n_delta or row >= 2^k is written as zero
+// and counted in *d_invalid (a device counter; may be null).
+int perm_sigmas_run(const uint32_t* d_map, size_t n_columns, uint32_t k, const Fr* h_tab, size_t n_delta, uint32_t lo_bits, Fr* d_out, size_t out_stride,
+                    unsigned long long* d_invalid, StagingRing& ring, cudaStream_t st);
 // out[p] = sum_i coeffs[p*stride + i] * x[p]^i   for p < batch (eval_polynomial); h_x host array, d_out device array
 int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_out, int batch, PolyWorkspace& ws, StagingRing& ring, cudaStream_t st);
 // in place a[i] <- a[i]^-1 (zeros stay zero)  (ff::BatchInvert)

@@ -243,6 +243,26 @@ def kate_division(a: torch.Tensor, b, out: torch.Tensor | None = None) -> torch.
     return out
 
 
+def permutation_sigmas(mapping: torch.Tensor, k: int, out: torch.Tensor | None = None, count_invalid: bool = False):
+    """Sigma columns from the copy-constraint mapping (int32 [P, 2^k, 2], (column, row) per cell) -> out [P, m, 4] with m >= 2^k (rows
+    beyond 2^k untouched).  Cells outside P columns x 2^k rows are written as zero; with count_invalid the call synchronises and returns
+    (out, number of such cells)."""
+    from .evaluation import DELTA
+    assert mapping.is_cuda and mapping.dtype == torch.int32 and mapping.is_contiguous() and mapping.dim() == 3 and mapping.shape[1:] == (1 << k, 2), \
+        (mapping.dtype, mapping.shape)
+    nat.ensure_init()
+    P = mapping.shape[0]
+    if out is None:
+        out = torch.empty((P, 1 << k, 4), dtype=torch.int64, device=mapping.device)
+    _chk(out, 4)
+    assert out.dim() == 3 and out.shape[0] == P, out.shape
+    omega = F.fr_to_limbs(pow(F.FR_ROOT_OF_UNITY, 1 << (F.FR_S - k), F.FR_MODULUS))
+    invalid = C.c_uint64(0)
+    nat.check(nat.lib().b200_permutation_sigmas_dev(mapping.data_ptr(), P, k, nat.ptr(omega), nat.ptr(F.fr_to_limbs(DELTA)), out.data_ptr(), out.shape[1],
+                                                    C.byref(invalid) if count_invalid else None, _stream()))
+    return (out, invalid.value) if count_invalid else out
+
+
 def to_host(t: torch.Tensor) -> np.ndarray:
     return t.cpu().numpy().view(np.uint64)
 

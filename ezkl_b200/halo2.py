@@ -365,6 +365,23 @@ class ParamsKZG:
 
 
 # ------------------------------------------------------------------------------------------------------------
+# plonk/permutation/keygen.rs
+def permutation_sigmas(mapping, k: int) -> np.ndarray:
+    """Assembly::build_pk's sigma columns: mapping [P, 2^k, 2] uint32 (column, row) per cell, the Assembly's mapping after its cycles are
+    merged -> [P, 2^k, 4], cell (j, i) = DELTA^column * omega^row.  A cell outside P columns x 2^k rows raises B200Error."""
+    from .evaluation import DELTA
+    m = np.ascontiguousarray(mapping, dtype=np.uint32)
+    P = m.shape[0]
+    assert m.shape == (P, 1 << k, 2), m.shape
+    out = np.zeros((P, 1 << k, 4), np.uint64)
+    nat.ensure_init()
+    omega = F.fr_to_limbs(pow(F.FR_ROOT_OF_UNITY, 1 << (F.FR_S - k), F.FR_MODULUS))
+    nat.check(nat.lib().b200_permutation_sigmas(m.ctypes.data_as(C.c_void_p), P, k, nat.ptr(omega), nat.ptr(F.fr_to_limbs(DELTA)),
+                                                nat.ptr_array([out[j] for j in range(P)]) if P else None))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------
 # plonk/keygen.rs + plonk.rs ProvingKey (RawBytes layout, SURVEY.md Appendix B)
 class ProvingKey:
     """ProvingKey<G1Affine> as `ProvingKey::write(.., SerdeFormat::RawBytes)` lays it out (what src/pfsys/mod.rs:615-636 loads):
