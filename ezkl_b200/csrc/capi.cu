@@ -18,6 +18,7 @@
 #include "../../include/ezkl_b200.h"
 #include "../../include/ezkl_b200_keygen.h"
 #include "../../include/ezkl_b200_resident.h"
+#include "../../include/ezkl_b200_srs.h"
 #include "msm.cuh"
 #include "ntt.cuh"
 #include "poly.cuh"
@@ -639,27 +640,28 @@ int b200_sync_all(void) {
 }
 
 // ---- bases ---------------------------------------------------------------------------------------------------
-// The bases come from the device (d_bases, copied into level 0) or from the host (h_bases, uploaded straight into level 0 of the
-// new table, so no staging buffer of the calling thread grows to the size of an SRS vector).  max_table_bytes = 0: the configured budget.
-static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, const b200_g1_affine* h_bases, size_t n, int window_bits, size_t max_table_bytes,
-                             uint64_t* handle) {
-    B200_CHECK((d_bases || h_bases) && handle && n > 0, -1, "bases_register: null argument or n == 0");
-    B200_CHECK(window_bits == 0 || (window_bits >= 4 && window_bits <= 24), -1, "bases_register: window_bits %d not in {0, 4..24}", window_bits);
+// Registration in the steps that b200_bases_register* and b200_srs_register share: bases_alloc makes a BaseSet whose table on the
+// context's device is allocated with level 0 left for the caller to fill, bases_build fills the other levels and enqueues the replica
+// copies, bases_drop is the failure cleanup (it frees every table of the set) and bases_publish hands out the handle once the stream
+// has finished.  `who` names the entry point in the error messages.
+static int bases_drop(BaseSet* bs, int rc) {
+    int cur = 0; cudaGetDevice(&cur);
+    for (int s = 0; s < MAX_DEV; ++s) if (bs->t[s]) { cudaSetDevice(bs->t[s]->device); msm_table_free(bs->t[s]); delete bs->t[s]; }
+    cudaSetDevice(cur);
+    delete bs; return rc;
+}
+static int bases_alloc(Ctx* c, size_t n, int window_bits, size_t max_table_bytes, BaseSet** out) {
     BaseSet* bs = new BaseSet();
-    auto fail = [&](int rc) {
-        int cur = 0; cudaGetDevice(&cur);
-        for (int s = 0; s < MAX_DEV; ++s) if (bs->t[s]) { cudaSetDevice(bs->t[s]->device); msm_table_free(bs->t[s]); delete bs->t[s]; }
-        cudaSetDevice(cur);
-        delete bs; return rc;
-    };
     MsmTable* t = new MsmTable();
     bs->t[c->slot] = t;
-    if (int rc = msm_table_alloc(t, n, window_bits, max_table_bytes ? max_table_bytes : config().msm_table_budget)) return fail(rc);
-    if (h_bases) {
-        if (int rc = h2d_one(c, t->d_table, h_bases, sizeof(G1Affine) * n, st)) return fail(rc);
-    }
-    if (int rc = msm_table_build(t, reinterpret_cast<const G1Affine*>(d_bases), st)) return fail(rc);
-    bs->n = n; bs->c = t->c; bs->W = t->W; bs->s = t->s; bs->L = t->L;
+    if (int rc = msm_table_alloc(t, n, window_bits, max_table_bytes ? max_table_bytes : config().msm_table_budget)) return bases_drop(bs, rc);
+    *out = bs;
+    return 0;
+}
+static int bases_build(Ctx* c, cudaStream_t st, BaseSet* bs, const void* d_bases, const char* who) {
+    MsmTable* t = bs->t[c->slot];
+    if (int rc = msm_table_build(t, reinterpret_cast<const G1Affine*>(d_bases), st)) return rc;
+    bs->n = t->n; bs->c = t->c; bs->W = t->W; bs->s = t->s; bs->L = t->L;
     // replicas: the finished table crosses NVLink once per extra device (cheaper than rebuilding: one inversion per point and level)
     for (int s = 0; s < g_ndev.load(); ++s) if (s != c->slot) {
         MsmTable* r = new MsmTable();
@@ -668,15 +670,33 @@ static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, const
         cudaSetDevice(r->device);
         cudaError_t e = cudaMalloc(&r->d_table, t->bytes());
         cudaSetDevice(c->dev);
-        if (e != cudaSuccess) { set_error("bases_register: replica on device %d: %s", r->device, cudaGetErrorString(e)); return fail(-2); }
+        if (e != cudaSuccess) { set_error("%s: replica on device %d: %s", who, r->device, cudaGetErrorString(e)); return -2; }
         e = cudaMemcpyPeerAsync(r->d_table, r->device, t->d_table, t->device, t->bytes(), st);
-        if (e != cudaSuccess) { set_error("bases_register: peer copy: %s", cudaGetErrorString(e)); return fail(-2); }
+        if (e != cudaSuccess) { set_error("%s: peer copy: %s", who, cudaGetErrorString(e)); return -2; }
     }
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error("bases_register: %s", cudaGetErrorString(e)); return fail(-2); }
+    return 0;
+}
+static uint64_t bases_publish(BaseSet* bs) {
     std::lock_guard<std::mutex> lk(g_mu);
-    *handle = g_next_handle++;
-    g_tables[*handle] = bs;
+    const uint64_t h = g_next_handle++;
+    g_tables[h] = bs;
+    return h;
+}
+// The bases come from the device (d_bases, copied into level 0) or from the host (h_bases, uploaded straight into level 0 of the
+// new table, so no staging buffer of the calling thread grows to the size of an SRS vector).  max_table_bytes = 0: the configured budget.
+static int bases_register_on(Ctx* c, cudaStream_t st, const void* d_bases, const b200_g1_affine* h_bases, size_t n, int window_bits, size_t max_table_bytes,
+                             uint64_t* handle) {
+    B200_CHECK((d_bases || h_bases) && handle && n > 0, -1, "bases_register: null argument or n == 0");
+    B200_CHECK(window_bits == 0 || (window_bits >= 4 && window_bits <= 24), -1, "bases_register: window_bits %d not in {0, 4..24}", window_bits);
+    BaseSet* bs = nullptr;
+    if (int rc = bases_alloc(c, n, window_bits, max_table_bytes, &bs)) return rc;
+    if (h_bases) {
+        if (int rc = h2d_one(c, bs->t[c->slot]->d_table, h_bases, sizeof(G1Affine) * n, st)) return bases_drop(bs, rc);
+    }
+    if (int rc = bases_build(c, st, bs, d_bases, "bases_register")) return bases_drop(bs, rc);
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { set_error("bases_register: %s", cudaGetErrorString(e)); return bases_drop(bs, -2); }
+    *handle = bases_publish(bs);
     return 0;
 }
 int b200_bases_register_ex_dev(const void* d_bases, size_t n, int window_bits, size_t max_table_bytes, uint64_t* handle) {
@@ -1542,6 +1562,65 @@ int b200_evaluate_h_dev(const void* const* d_polys, const size_t* lengths, size_
                                      loads, n_loads, constants, n_constants, program, n_instr, c->stage_c.as<Fr>(), c->stage_b.as<Fr>(), h, nullptr)) return rc;
     if (!t_evaluations) return 0;
     return evaluate_h_finish(c, ss.st, h, c->stage_b.as<Fr>(), ext_k, zeta, t_evaluations, t_period, ext_omega_inv, ext_ifft_divisor);
+}
+
+// ---- SRS (include/ezkl_b200_srs.h) ------------------------------------------------------------------------------------------------
+// Fr's 2^28-th root of unity (halo2curves Fr::ROOT_OF_UNITY = 7^((r - 1) / 2^28)) in Montgomery form
+static Fr fr_root_of_unity() {
+    Fr w;
+    const uint32_t v[8] = {0x60c37c9cu, 0xd34f1ed9u, 0xd39329c8u, 0x3215cf6du, 0x3dd31f74u, 0x98865ea9u, 0x166d18b7u, 0x03ddb9f5u};
+    memcpy(w.l, v, sizeof v);
+    return fp_to_mont(w);
+}
+static const char* g1_invalid_reason(unsigned r) {
+    return r == G1_X_NOT_CANONICAL ? "x is not below p" : r == G1_Y_NOT_CANONICAL ? "y is not below p" : "is not on the curve";
+}
+// Both vectors go straight into level 0 of their new tables and are checked there; only when every point passed is valid does the group
+// FFT (for a NULL g_lagrange) run, from level 0 of g's table into level 0 of the other, so a rejected file costs no FFT scratch.
+static int srs_register_on(Ctx* c, cudaStream_t st, const b200_g1_affine* g, const b200_g1_affine* gl, uint32_t k, int window_bits, size_t max_table_bytes,
+                           uint64_t* g_handle, uint64_t* g_lagrange_handle) {
+    const size_t n = (size_t)1 << k;
+    BaseSet* bs[2] = {nullptr, nullptr};
+    auto fail = [&](int rc) { for (BaseSet* b : bs) if (b) bases_drop(b, rc); return rc; };
+    auto cuda_fail = [&](cudaError_t e) { set_error("srs_register: %s", cudaGetErrorString(e)); return fail(-2); };
+    for (int v = 0; v < 2; ++v) if (int rc = bases_alloc(c, n, window_bits, max_table_bytes, &bs[v])) return fail(rc);
+    G1Affine* lv0[2] = {bs[0]->t[c->slot]->d_table, bs[1]->t[c->slot]->d_table};
+    const b200_g1_affine* src[2] = {g, gl};
+    if (c->small.ensure(2 * sizeof(unsigned long long))) return fail(-2);
+    unsigned long long* d_first = c->small.as<unsigned long long>();
+    if (cudaError_t e = cudaMemsetAsync(d_first, 0xff, 2 * sizeof(unsigned long long), st)) return cuda_fail(e);
+    for (int v = 0; v < 2; ++v) if (src[v]) {
+        if (int rc = h2d_one(c, lv0[v], src[v], sizeof(G1Affine) * n, st)) return fail(rc);
+        if (int rc = g1_validate_run(lv0[v], n, d_first + v, st)) return fail(rc);
+    }
+    unsigned long long first[2];
+    if (cudaError_t e = cudaMemcpyAsync(first, d_first, sizeof first, cudaMemcpyDeviceToHost, st)) return cuda_fail(e);
+    if (cudaError_t e = cudaStreamSynchronize(st)) return cuda_fail(e);
+    for (int v = 0; v < 2; ++v) if (first[v] != ~0ull) {
+        set_error("srs_register: %s[%llu] %s", v ? "g_lagrange" : "g", first[v] >> 2, g1_invalid_reason((unsigned)(first[v] & 3)));
+        return fail(-1);
+    }
+    if (!gl) {                                  // ParamsKZG::downsize: g_lagrange = n^-1 * FFT_{omega^-1}(g)
+        Fr w = fr_root_of_unity();
+        for (uint32_t i = k; i < 28; ++i) w = w * w;
+        Fr nf = fp_zero<FrTag>(); nf.l[0] = (uint32_t)n;
+        const Fr w_inv = fp_inv(w), n_inv = fp_inv(fp_to_mont(nf));
+        if (int rc = g1_fft_on(c, st, lv0[0], k, reinterpret_cast<const b200_fr*>(&w_inv), reinterpret_cast<const b200_fr*>(&n_inv), lv0[1])) return fail(rc);
+    }
+    for (int v = 0; v < 2; ++v) if (int rc = bases_build(c, st, bs[v], nullptr, "srs_register")) return fail(rc);
+    if (cudaError_t e = cudaStreamSynchronize(st)) return cuda_fail(e);
+    *g_handle = bases_publish(bs[0]);
+    *g_lagrange_handle = bases_publish(bs[1]);
+    return 0;
+}
+int b200_srs_register(const b200_g1_affine* g, const b200_g1_affine* g_lagrange, uint32_t k, int window_bits, size_t max_table_bytes,
+                      uint64_t* g_handle, uint64_t* g_lagrange_handle) {
+    B200_ENTER(c, nullptr);
+    B200_CHECK(g && g_handle && g_lagrange_handle, -1, "srs_register: null argument (g, g_handle and g_lagrange_handle are required)");
+    B200_CHECK(k <= 26, -1, "srs_register: k = %u out of range [0, 26]", k);
+    B200_CHECK(window_bits == 0 || (window_bits >= 4 && window_bits <= 24), -1, "srs_register: window_bits %d not in {0, 4..24}", window_bits);
+    StreamScope ss(c, nullptr);
+    return srs_register_on(c, ss.st, g, g_lagrange, k, window_bits, max_table_bytes, g_handle, g_lagrange_handle);
 }
 
 }  // extern "C"

@@ -7,6 +7,7 @@
 // Radix-2 decimation-in-time on XYZZ points in global memory, one kernel per stage; each butterfly multiplies its odd input by
 // a 254-bit twiddle with a 4-bit fixed-window ladder (the table of 1..15 multiples lives in the thread's local memory).
 // Bound: n/2 * log n * ~3000 field multiplications — pure multiply issue, like everything else here.
+// Also here: k_g1_validate, the point check of an SRS vector read from a file (b200_srs_register, include/ezkl_b200_srs.h).
 #include "msm.cuh"
 
 namespace b200 {
@@ -56,6 +57,35 @@ __global__ void __launch_bounds__(128) k_ecfft_store(const G1Xyzz* __restrict__ 
 __global__ void k_powers_fr(Fr base, uint32_t count, Fr* __restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count) fp_store(out + i, fp_pow_u64(base, (uint64_t)i));
+}
+
+// SRS point check (halo2curves G1Affine::from_raw_bytes, as ParamsKZG::read in RawBytes form applies it to every point it reads):
+// both coordinates canonical (the 256-bit limb integer below p), and (x, y) = (0, 0) or y^2 = x^3 + 3 in Montgomery form.  One thread
+// per point, 64 B read and 2 squarings + 1 multiplication; the first failure is kept as min(index << 2 | reason) in *first.
+DEV bool fq_is_canonical(const Fq& a) {
+#pragma unroll
+    for (int i = 7; i >= 0; --i) if (a.l[i] != FqTag::mod(i)) return a.l[i] < FqTag::mod(i);
+    return false;
+}
+__global__ void __launch_bounds__(256) k_g1_validate(const G1Affine* __restrict__ pts, size_t n, unsigned long long* __restrict__ first) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    G1Affine p;
+    p.x = fp_load(&pts[i].x); p.y = fp_load(&pts[i].y);
+    unsigned reason = G1_VALID;
+    if (!fq_is_canonical(p.x)) reason = G1_X_NOT_CANONICAL;
+    else if (!fq_is_canonical(p.y)) reason = G1_Y_NOT_CANONICAL;
+    else if (!g1_is_identity(p)) {
+        const Fq b = fp_one<FqTag>() + fp_one<FqTag>() + fp_one<FqTag>();         // 3 R mod p
+        if (!fp_eq(fp_sqr(p.y), fp_sqr(p.x) * p.x + b)) reason = G1_NOT_ON_CURVE;
+    }
+    if (reason != G1_VALID) atomicMin(first, ((unsigned long long)i << 2) | reason);
+}
+int g1_validate_run(const G1Affine* d_pts, size_t n, unsigned long long* d_first, cudaStream_t st) {
+    if (n == 0) return 0;
+    k_g1_validate<<<div_up(n, 256), 256, 0, st>>>(d_pts, n, d_first); count_launch();
+    B200_CUDA(cudaGetLastError());
+    return 0;
 }
 
 int g1_fft_run(const G1Affine* d_in, uint32_t log_n, const Fr& omega, const Fr* scale /*nullable*/, G1Affine* d_out, DevBuf& scratch, cudaStream_t st) {

@@ -144,6 +144,10 @@ int msm_run(const MsmTable& t, const Fr* d_scalars, size_t n, size_t stride, int
 int g1_fixed_base_mul_run(const Fr* d_scalars, size_t n, const G1Affine& base, G1Affine* d_out, cudaStream_t st);
 // out[j] = scale * sum_i omega^(i j) * P_i over G1 (halo2 g_to_lagrange / ParamsKZG::downsize); affine in, affine out
 int g1_fft_run(const G1Affine* d_in, uint32_t log_n, const Fr& omega, const Fr* scale, G1Affine* d_out, DevBuf& scratch, cudaStream_t st);
+// SRS point check (k_g1_validate): a point is valid when x and y are canonical and it is (0, 0) or on y^2 = x^3 + 3.  For every
+// invalid point i, *d_first = min(*d_first, i << 2 | reason); the caller sets *d_first to ~0 first.
+enum G1Invalid : unsigned { G1_X_NOT_CANONICAL = 0, G1_Y_NOT_CANONICAL = 1, G1_NOT_ON_CURVE = 2, G1_VALID = 3 };
+int g1_validate_run(const G1Affine* d_pts, size_t n, unsigned long long* d_first, cudaStream_t st);
 int g1_generate_run(uint64_t seed, size_t n, G1Affine* d_out, cudaStream_t st);
 // out[g] = sum_j points[g*count + j]
 int g1_sum_run(const G1Xyzz* d_points, size_t groups, size_t count, G1Xyzz* d_out, cudaStream_t st);

@@ -49,6 +49,14 @@ class Bases:
         self.handle = h.value
         return self
 
+    @classmethod
+    def from_handle(cls, handle: int):
+        """Wraps a handle the library registered (b200_srs_register); release() gives it back."""
+        self = cls.__new__(cls)
+        self.handle = handle
+        self.n = bases_info(handle)["n"]
+        return self
+
     def info(self):
         return bases_info(self.handle)
 
@@ -56,6 +64,37 @@ class Bases:
         if self.handle:
             nat.check(nat.lib().b200_bases_release(self.handle))
             self.handle = 0
+
+
+def srs_bases(path: str, k: int, window_bits: int = 0, max_table_bytes: int = 0):
+    """A KZG parameter file (ParamsKZG::write layout: u32 LE k_file | g | g_lagrange | G2 tail) -> (Bases of g[:2^k], Bases of the
+    Lagrange-basis key for k), through b200_srs_register: the file is memory-mapped, only g[:2^k] (and g_lagrange when k == k_file) is read,
+    every point passed is checked on the device, and for k < k_file the Lagrange-basis key is computed on the device as
+    ParamsKZG::downsize computes it.  A file whose length is not that of its header's k, or k > k_file, raises before the library is
+    called."""
+    import os
+    size = os.path.getsize(path)
+    with open(path, "rb") as f:
+        head = f.read(4)
+    if len(head) < 4:
+        raise nat.B200Error("srs_bases: %s has %d bytes, no header" % (path, size))
+    (k_file,) = struct.unpack("<I", head)
+    if k_file > 32 or size != 4 + 128 * (1 << k_file) + 256:
+        raise nat.B200Error("srs_bases: %d bytes, expected %d for k=%d" % (size, 4 + 128 * (1 << min(k_file, 32)) + 256, k_file))
+    if not 0 <= k <= k_file:
+        raise nat.B200Error("srs_bases: k = %d not in [0, k_file = %d]" % (k, k_file))
+    n, n_file = 1 << k, 1 << k_file
+    mm = np.memmap(path, dtype="<u8", mode="r", offset=4, shape=(2 * n_file, 8))
+    g = mm[:n]
+    gl = mm[n_file:n_file + n] if k == k_file else None
+    nat.ensure_init()
+    hg, hl = C.c_uint64(0), C.c_uint64(0)
+    try:
+        nat.check(nat.lib().b200_srs_register(g.ctypes.data, None if gl is None else gl.ctypes.data, k, window_bits, max_table_bytes,
+                                               C.byref(hg), C.byref(hl)))
+    finally:
+        del g, gl, mm
+    return Bases.from_handle(hg.value), Bases.from_handle(hl.value)
 
 
 def bases_info(handle: int) -> dict:
