@@ -1,5 +1,5 @@
-"""ctypes binding of libezkl_b200.so (the C ABI in include/ezkl_b200.h, include/ezkl_b200_resident.h, include/ezkl_b200_keygen.h and
-include/ezkl_b200_srs.h).
+"""ctypes binding of libezkl_b200.so (the C ABI in include/ezkl_b200.h, include/ezkl_b200_resident.h, include/ezkl_b200_keygen.h,
+include/ezkl_b200_srs.h and include/ezkl_b200_pk.h).
 
 There is no fallback: if the shared library is missing, or b200_init finds no sm_90 device, the error is raised to the
 caller.  Arrays are numpy uint64 in the wire format (Fr -> [...,4], G1Affine -> [...,8], G1 Jacobian -> [...,12],
@@ -22,6 +22,7 @@ HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200.h")
 RESIDENT_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_resident.h")     # entry points for device-resident callers
 KEYGEN_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_keygen.h")         # key-generation entry points
 SRS_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_srs.h")               # SRS file -> registered base tables
+PK_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_pk.h")                 # proving-key file -> device columns
 DBG_LIB_PATH = os.path.join(_HERE, "libezkl_b200_dbg.so")
 DBG_HEADER = os.path.join(_HERE, "csrc", "debug.h")
 
@@ -83,7 +84,7 @@ _inited = False
 def lib():
     global _lib
     if _lib is None:
-        _lib = _load(LIB_PATH, (HEADER, RESIDENT_HEADER, KEYGEN_HEADER, SRS_HEADER), "`python -c 'import __graft_entry__ as g; g.build()'` or `make -C ezkl_b200/csrc`")
+        _lib = _load(LIB_PATH, (HEADER, RESIDENT_HEADER, KEYGEN_HEADER, SRS_HEADER, PK_HEADER), "`python -c 'import __graft_entry__ as g; g.build()'` or `make -C ezkl_b200/csrc`")
     return _lib
 
 

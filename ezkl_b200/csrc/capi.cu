@@ -17,6 +17,7 @@
 
 #include "../../include/ezkl_b200.h"
 #include "../../include/ezkl_b200_keygen.h"
+#include "../../include/ezkl_b200_pk.h"
 #include "../../include/ezkl_b200_resident.h"
 #include "../../include/ezkl_b200_srs.h"
 #include "msm.cuh"
@@ -1572,6 +1573,18 @@ static Fr fr_root_of_unity() {
     memcpy(w.l, v, sizeof v);
     return fp_to_mont(w);
 }
+// the 2^log_n-th root of unity of halo2's EvaluationDomain, ROOT_OF_UNITY^(2^(28 - log_n)), log_n <= 28
+static Fr fr_omega(uint32_t log_n) {
+    Fr w = fr_root_of_unity();
+    for (uint32_t i = log_n; i < 28; ++i) w = w * w;
+    return w;
+}
+// 1 / x for a small integer x, Montgomery form
+static Fr fr_inv_u64(uint64_t x) {
+    Fr f = fp_zero<FrTag>();
+    f.l[0] = (uint32_t)x; f.l[1] = (uint32_t)(x >> 32);
+    return fp_inv(fp_to_mont(f));
+}
 static const char* g1_invalid_reason(unsigned r) {
     return r == G1_X_NOT_CANONICAL ? "x is not below p" : r == G1_Y_NOT_CANONICAL ? "y is not below p" : "is not on the curve";
 }
@@ -1601,10 +1614,7 @@ static int srs_register_on(Ctx* c, cudaStream_t st, const b200_g1_affine* g, con
         return fail(-1);
     }
     if (!gl) {                                  // ParamsKZG::downsize: g_lagrange = n^-1 * FFT_{omega^-1}(g)
-        Fr w = fr_root_of_unity();
-        for (uint32_t i = k; i < 28; ++i) w = w * w;
-        Fr nf = fp_zero<FrTag>(); nf.l[0] = (uint32_t)n;
-        const Fr w_inv = fp_inv(w), n_inv = fp_inv(fp_to_mont(nf));
+        const Fr w_inv = fp_inv(fr_omega(k)), n_inv = fr_inv_u64(n);
         if (int rc = g1_fft_on(c, st, lv0[0], k, reinterpret_cast<const b200_fr*>(&w_inv), reinterpret_cast<const b200_fr*>(&n_inv), lv0[1])) return fail(rc);
     }
     for (int v = 0; v < 2; ++v) if (int rc = bases_build(c, st, bs[v], nullptr, "srs_register")) return fail(rc);
@@ -1621,6 +1631,100 @@ int b200_srs_register(const b200_g1_affine* g, const b200_g1_affine* g_lagrange,
     B200_CHECK(window_bits == 0 || (window_bits >= 4 && window_bits <= 24), -1, "srs_register: window_bits %d not in {0, 4..24}", window_bits);
     StreamScope ss(c, nullptr);
     return srs_register_on(c, ss.st, g, g_lagrange, k, window_bits, max_table_bytes, g_handle, g_lagrange_handle);
+}
+
+// ---- proving key (include/ezkl_b200_pk.h) -----------------------------------------------------------------------------------------
+// Fr::ZETA (halo2curves), the cube root of unity that coeff_to_extended distributes as [1, zeta, zeta^2], in Montgomery form
+static Fr fr_zeta() {
+    Fr z;
+    const uint32_t v[8] = {0x36636f23u, 0xb8ca0b2du, 0xec2bc5e9u, 0xcc37a73fu, 0x3fd84104u, 0x048b6e19u, 0xe131a029u, 0x30644e72u};
+    memcpy(z.l, v, sizeof v);
+    return fp_to_mont(z);
+}
+// the device that owns a caller's buffer, or -1 when it is not device memory
+static int device_of(const void* p) {
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return -1; }
+    return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged ? at.device : -1;
+}
+// cols[j] (j < n_cols, fixed columns first) -> values, checked; only when every element passed is canonical are polys and l written.
+// polys: iNTT (omega^-1, then 2^-k) of the values in column groups bounded by the call budget.  l: the Lagrange indicators of rows {0},
+// {u} and [0, u) -- whose interpolants are L_0, L_u and 1 - L_u - sum_{r > u} L_r -- to coefficients, then coeff_to_extended.
+static int pk_load_on(Ctx* c, cudaStream_t st, const void* const* cols, size_t n_cols, size_t n_fixed, uint32_t k, uint32_t ext_k, uint32_t blinding_factors,
+                      Fr* values, Fr* polys, size_t stride, Fr* l) {
+    const size_t n = (size_t)1 << k, N = (size_t)1 << ext_k;
+    if (c->small.ensure(sizeof(unsigned long long))) return -2;
+    unsigned long long* d_first = c->small.as<unsigned long long>();
+    B200_CUDA(cudaMemsetAsync(d_first, 0xff, sizeof *d_first, st));
+    for (size_t j = 0; j < n_cols; ++j) {               // column j's check runs while the host stages column j + 1
+        if (int rc = h2d_one(c, values + j * stride, cols[j], sizeof(Fr) * n, st)) return rc;
+        if (int rc = fr_validate_run(values + j * stride, n, j, d_first, st)) return rc;
+    }
+    unsigned long long first = ~0ull;
+    B200_CUDA(cudaMemcpyAsync(&first, d_first, sizeof first, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    if (first != ~0ull) {
+        const size_t col = (size_t)(first >> 32), row = (size_t)(first & 0xffffffffu);
+        set_error("pk_load: %s[%zu][%zu] is not below r", col < n_fixed ? "fixed_values" : "permutations", col < n_fixed ? col : col - n_fixed, row);
+        return -1;
+    }
+    const size_t budget = call_budget();
+    size_t g = budget / (sizeof(Fr) * n), s = budget / (sizeof(Fr) * N);
+    g = g < 1 ? 1 : (g > n_cols ? n_cols : (g > 65535 ? 65535 : g));
+    s = s < 1 ? 1 : (s > 3 ? 3 : s);
+    const size_t tmp_elems = g * n > s * N ? g * n : s * N;
+    if (c->stage_a.ensure(sizeof(Fr) * 3 * n) || c->stage_b.ensure(sizeof(Fr) * tmp_elems)) return -2;
+    Fr* coef = c->stage_a.as<Fr>();
+    Fr* tmp = c->stage_b.as<Fr>();
+    const Fr w_inv = fp_inv(fr_omega(k)), zeta = fr_zeta();
+    NttScale none, div_n, zeta_cycle;
+    div_n.mode = 1; div_n.c[0] = fr_inv_u64(n);
+    zeta_cycle.mode = 3; zeta_cycle.c[0] = fp_one<FrTag>(); zeta_cycle.c[1] = zeta; zeta_cycle.c[2] = zeta * zeta;
+    for (size_t j0 = 0; j0 < n_cols; j0 += g) {
+        const int nb = (int)(n_cols - j0 < g ? n_cols - j0 : g);
+        if (int rc = ntt_call(c, st, values + j0 * stride, stride, n, tmp, polys + j0 * stride, stride, k, w_inv, none, div_n, nb)) return rc;
+    }
+    const uint64_t u = n - blinding_factors - 1, lo[3] = {0, u, 0}, hi[3] = {1, u + 1, u};
+    if (int rc = fr_indicator_run(coef, n, lo, hi, st)) return rc;
+    for (size_t j0 = 0; j0 < 3; j0 += s) {
+        const int nb = (int)(3 - j0 < s ? 3 - j0 : s);
+        if (int rc = ntt_call(c, st, coef + j0 * n, n, n, tmp, coef + j0 * n, n, k, w_inv, none, div_n, nb)) return rc;
+        if (int rc = ntt_call(c, st, coef + j0 * n, n, n, tmp, l + j0 * N, N, ext_k, fr_omega(ext_k), zeta_cycle, none, nb)) return rc;
+    }
+    B200_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
+int b200_pk_load(const void* const* h_fixed_values, size_t n_fixed, const void* const* h_permutations, size_t n_perm, uint32_t k, uint32_t ext_k,
+                 uint32_t blinding_factors, void* d_values, void* d_polys, size_t stride, void* d_l) {
+    B200_ENTER(c, d_values ? d_values : d_l);
+    B200_CHECK(k >= 1 && ext_k >= k && ext_k <= 28, -1, "pk_load: need 1 <= k <= ext_k <= 28 (k = %u, ext_k = %u)", k, ext_k);
+    const size_t n = (size_t)1 << k, n_cols = n_fixed + n_perm;
+    B200_CHECK(blinding_factors < n, -1, "pk_load: blinding_factors = %u, need fewer than 2^k = %zu", blinding_factors, n);
+    B200_CHECK(stride >= n, -1, "pk_load: stride %zu < 2^k = %zu", stride, n);
+    B200_CHECK(n_cols < ((size_t)1 << 32) && (n_cols == 0 || stride <= ((size_t)1 << 58) / n_cols), -1, "pk_load: %zu columns of stride %zu exceed the address space",
+               n_cols, stride);
+    B200_CHECK(d_l && (n_cols == 0 || (d_values && d_polys)) && (n_fixed == 0 || h_fixed_values) && (n_perm == 0 || h_permutations), -1,
+               "pk_load: null pointer (d_l is required; d_values, d_polys and the column arrays may be NULL only when there are no columns)");
+    std::vector<const void*> cols(n_cols);
+    for (size_t j = 0; j < n_cols; ++j) {
+        cols[j] = j < n_fixed ? h_fixed_values[j] : h_permutations[j - n_fixed];
+        B200_CHECK(cols[j], -1, "pk_load: %s[%zu] is null", j < n_fixed ? "h_fixed_values" : "h_permutations", j < n_fixed ? j : j - n_fixed);
+    }
+    const char* names[3] = {"d_values", "d_polys", "d_l"};
+    const uintptr_t lo[3] = {(uintptr_t)d_values, (uintptr_t)d_polys, (uintptr_t)d_l};
+    const size_t col_bytes = n_cols ? sizeof(Fr) * ((n_cols - 1) * stride + n) : 0;
+    const uintptr_t hi[3] = {lo[0] + col_bytes, lo[1] + col_bytes, lo[2] + sizeof(Fr) * 3 * ((size_t)1 << ext_k)};
+    for (int a = 0; a < 3; ++a) {
+        if (hi[a] == lo[a]) continue;
+        B200_CHECK((lo[a] & 15) == 0, -1, "pk_load: %s is not 16-byte aligned", names[a]);
+        const int dev = device_of((const void*)lo[a]);
+        B200_CHECK(dev == c->dev, -1, dev < 0 ? "pk_load: %s is not device memory" : "pk_load: %s is on another device than the other outputs", names[a]);
+        for (int b = 0; b < a; ++b)
+            B200_CHECK(hi[b] == lo[b] || hi[a] <= lo[b] || lo[a] >= hi[b], -1, "pk_load: %s overlaps %s", names[a], names[b]);
+    }
+    StreamScope ss(c, nullptr);
+    return pk_load_on(c, ss.st, cols.data(), n_cols, n_fixed, k, ext_k, blinding_factors, reinterpret_cast<Fr*>(d_values), reinterpret_cast<Fr*>(d_polys),
+                      stride, reinterpret_cast<Fr*>(d_l));
 }
 
 }  // extern "C"

@@ -62,19 +62,14 @@ __global__ void k_powers_fr(Fr base, uint32_t count, Fr* __restrict__ out) {
 // SRS point check (halo2curves G1Affine::from_raw_bytes, as ParamsKZG::read in RawBytes form applies it to every point it reads):
 // both coordinates canonical (the 256-bit limb integer below p), and (x, y) = (0, 0) or y^2 = x^3 + 3 in Montgomery form.  One thread
 // per point, 64 B read and 2 squarings + 1 multiplication; the first failure is kept as min(index << 2 | reason) in *first.
-DEV bool fq_is_canonical(const Fq& a) {
-#pragma unroll
-    for (int i = 7; i >= 0; --i) if (a.l[i] != FqTag::mod(i)) return a.l[i] < FqTag::mod(i);
-    return false;
-}
 __global__ void __launch_bounds__(256) k_g1_validate(const G1Affine* __restrict__ pts, size_t n, unsigned long long* __restrict__ first) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     G1Affine p;
     p.x = fp_load(&pts[i].x); p.y = fp_load(&pts[i].y);
     unsigned reason = G1_VALID;
-    if (!fq_is_canonical(p.x)) reason = G1_X_NOT_CANONICAL;
-    else if (!fq_is_canonical(p.y)) reason = G1_Y_NOT_CANONICAL;
+    if (!fp_is_canonical(p.x)) reason = G1_X_NOT_CANONICAL;
+    else if (!fp_is_canonical(p.y)) reason = G1_Y_NOT_CANONICAL;
     else if (!g1_is_identity(p)) {
         const Fq b = fp_one<FqTag>() + fp_one<FqTag>() + fp_one<FqTag>();         // 3 R mod p
         if (!fp_eq(fp_sqr(p.y), fp_sqr(p.x) * p.x + b)) reason = G1_NOT_ON_CURVE;

@@ -191,6 +191,12 @@ template <class Tag> HD bool fp_eq(const Fp<Tag>& a, const Fp<Tag>& b) {
     return o == 0;
 }
 template <class Tag> HD Fp<Tag> fp_neg(const Fp<Tag>& a) { return fp_zero<Tag>() - a; }
+// the 8 limbs, read as one 256-bit integer, are below the modulus: the encoding check of halo2curves' from_raw_bytes, for Fr and Fq alike
+template <class Tag> HD bool fp_is_canonical(const Fp<Tag>& a) {
+#pragma unroll
+    for (int i = 7; i >= 0; --i) if (a.l[i] != Tag::mod(i)) return a.l[i] < Tag::mod(i);
+    return false;
+}
 // a*b + c*d and a*b - c*d with ONE Montgomery reduction on the device (fp_gen.py: gen_mul2, 466 instructions against
 // 312 + 312 + 25); the host build composes them from the single-product operators.
 template <class Tag> HD Fp<Tag> fp_muladd2(const Fp<Tag>& a, const Fp<Tag>& b, const Fp<Tag>& c, const Fp<Tag>& d) {

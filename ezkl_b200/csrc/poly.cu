@@ -139,6 +139,40 @@ int perm_sigmas_run(const uint32_t* d_map, size_t n_columns, uint32_t k, const F
     return 0;
 }
 
+// ---- proving-key load (b200_pk_load, include/ezkl_b200_pk.h) ----------------------------------------------------------------
+// The check of one key column as halo2curves' Fr::from_raw_bytes makes it: one thread per element, 32 B read and one limb comparison,
+// so HBM-bound.  Rows of a warp are consecutive, so its lowest failing lane is its lowest failing row: one atomicMin per warp at most,
+// on (column << 32 | row), which keeps the lowest (column, row) of the call.
+__global__ void __launch_bounds__(256) k_fr_validate(const Fr* __restrict__ col, size_t n, unsigned long long column, unsigned long long* __restrict__ first) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool bad = i < n && !fp_is_canonical(fp_load(col + i));
+    const unsigned lanes = __ballot_sync(0xffffffffu, bad);
+    if (lanes && (threadIdx.x & 31) == (unsigned)(__ffs(lanes) - 1)) atomicMin(first, (column << 32) | i);
+}
+int fr_validate_run(const Fr* d_col, size_t n, size_t column, unsigned long long* d_first, cudaStream_t st) {
+    B200_CHECK(n <= ((size_t)1 << 32) && column < ((size_t)1 << 32), -1, "fr_validate: bad argument");
+    if (n == 0) return 0;
+    k_fr_validate<<<div_up(n, 256), 256, 0, st>>>(d_col, n, column, d_first); count_launch();
+    B200_CUDA(cudaGetLastError());
+    return 0;
+}
+// out[j * n + i] = 1 (Montgomery) for lo[j] <= i < hi[j], else 0, for the three columns j < 3
+struct FrRanges { uint64_t lo[3], hi[3]; };
+__global__ void __launch_bounds__(256) k_fr_indicator(Fr* __restrict__ out, size_t n, FrRanges r) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned j = blockIdx.y;
+    const uint64_t lo = j == 0 ? r.lo[0] : (j == 1 ? r.lo[1] : r.lo[2]), hi = j == 0 ? r.hi[0] : (j == 1 ? r.hi[1] : r.hi[2]);   // no local copy of r
+    if (i < n) fp_store(out + j * n + i, i >= lo && i < hi ? fp_one<FrTag>() : fp_zero<FrTag>());
+}
+int fr_indicator_run(Fr* d_out, size_t n, const uint64_t lo[3], const uint64_t hi[3], cudaStream_t st) {
+    if (n == 0) return 0;
+    FrRanges r;
+    for (int j = 0; j < 3; ++j) { r.lo[j] = lo[j]; r.hi[j] = hi[j]; }
+    k_fr_indicator<<<dim3(div_up(n, 256), 3), 256, 0, st>>>(d_out, n, r); count_launch();
+    B200_CUDA(cudaGetLastError());
+    return 0;
+}
+
 // ---- shared-memory helpers for one Fr per thread -------------------------------------------------------------
 DEV Fr shf_get(const Fr* sh, uint32_t i) { return fp_load(sh + i); }
 DEV void shf_put(Fr* sh, uint32_t i, const Fr& v) { fp_store(sh + i, v); }

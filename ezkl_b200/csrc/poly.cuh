@@ -28,6 +28,11 @@ int poly_coset_fold(const FoldCol* d_cols, size_t n_cols, const Fr* d_tab, uint3
 // and counted in *d_invalid (a device counter; may be null).
 int perm_sigmas_run(const uint32_t* d_map, size_t n_columns, uint32_t k, const Fr* h_tab, size_t n_delta, uint32_t lo_bits, Fr* d_out, size_t out_stride,
                     unsigned long long* d_invalid, StagingRing& ring, cudaStream_t st);
+// proving-key column check (k_fr_validate): for every element i < n of d_col that is not canonical (its limb integer not below r),
+// *d_first = min(*d_first, column << 32 | i); the caller sets *d_first to ~0 first.  n <= 2^32, column < 2^32.
+int fr_validate_run(const Fr* d_col, size_t n, size_t column, unsigned long long* d_first, cudaStream_t st);
+// three Lagrange indicator columns of n elements at d_out (column j at d_out + j n): 1 on rows lo[j] <= i < hi[j], 0 elsewhere
+int fr_indicator_run(Fr* d_out, size_t n, const uint64_t lo[3], const uint64_t hi[3], cudaStream_t st);
 // out[p] = sum_i coeffs[p*stride + i] * x[p]^i   for p < batch (eval_polynomial); h_x host array, d_out device array
 int poly_eval(const Fr* coeffs, size_t stride, size_t n, const Fr* h_x, Fr* d_out, int batch, PolyWorkspace& ws, StagingRing& ring, cudaStream_t st);
 // in place a[i] <- a[i]^-1 (zeros stay zero)  (ff::BatchInvert)

@@ -263,6 +263,45 @@ def permutation_sigmas(mapping: torch.Tensor, k: int, out: torch.Tensor | None =
     return (out, invalid.value) if count_invalid else out
 
 
+class DeviceProvingKey:
+    """What the resident prover needs of a proving key, on the device: values / polys [num_fixed + num_permutation, 2^k, 4] (fixed columns
+    first), l0 / l_last / l_active_row [2^ext_k, 4], and the vk bytes of the file."""
+
+    def __init__(self, k, ext_k, num_fixed, vk_bytes, values, polys, l):
+        self.k, self.ext_k, self.num_fixed, self.vk_bytes = k, ext_k, num_fixed, vk_bytes
+        self.values, self.polys = values, polys
+        self.l0, self.l_last, self.l_active_row = l[0], l[1], l[2]
+
+
+def load_proving_key(path: str, num_permutation_columns: int, num_selectors: int, ext_k: int, blinding_factors: int) -> DeviceProvingKey:
+    """A RawBytes proving key file (ProvingKey::write) -> DeviceProvingKey, through b200_pk_load: the file is memory-mapped, its section
+    headers are walked (halo2.ProvingKey.layout: only the u32 counts and lengths are read), and only the fixed_values and permutations
+    columns are passed to the library, which checks every element on the device and derives the polys and l-cosets there.  The file's
+    polys, cosets and l-vectors are never read.  A malformed file raises B200Error before the library is called."""
+    from .halo2 import ProvingKey
+    import os
+    if os.path.getsize(path) == 0:
+        raise nat.B200Error("load_proving_key: %s is empty" % path)
+    mm = np.memmap(path, dtype=np.uint8, mode="r")
+    try:
+        lay = ProvingKey.layout(mm, num_permutation_columns, num_selectors, ext_k)
+        k = lay["k"]
+        nf, cols = len(lay["fixed_values"]), lay["fixed_values"] + lay["permutations"]
+        nat.ensure_init()
+        values = torch.empty((len(cols), 1 << k, 4), dtype=torch.int64, device="cuda")
+        polys = torch.empty_like(values)
+        l = torch.empty((3, 1 << ext_k, 4), dtype=torch.int64, device="cuda")
+        base = mm.ctypes.data
+        ptrs = lambda offs: (C.c_void_p * len(offs))(*[base + o for o in offs]) if offs else None
+        torch.cuda.current_stream().synchronize()          # the allocations' stream work is done before the library's stream writes them
+        nat.check(nat.lib().b200_pk_load(ptrs(lay["fixed_values"]), nf, ptrs(lay["permutations"]), len(cols) - nf, k, ext_k, blinding_factors,
+                                         values.data_ptr() if cols else None, polys.data_ptr() if cols else None, 1 << k, l.data_ptr()))
+        vk = bytes(mm[:lay["vk_len"]])
+    finally:
+        del mm
+    return DeviceProvingKey(k, ext_k, nf, vk, values, polys, l)
+
+
 def to_host(t: torch.Tensor) -> np.ndarray:
     return t.cpu().numpy().view(np.uint64)
 

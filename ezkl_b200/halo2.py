@@ -478,6 +478,84 @@ class ProvingKey:
             raise nat.B200Error("ProvingKey::read: %d trailing bytes (wrong column counts?)" % (len(d) - off))
         return pk
 
+    def _chunks(self):
+        """The file's bytes in write order, one section header or column at a time."""
+        poly = lambda p: (struct.pack(">I", len(p)), np.ascontiguousarray(p, "<u8").tobytes())
+        yield self.vk_bytes
+        for p in (self.l0, self.l_last, self.l_active_row):
+            yield from poly(p)
+        for ps in (self.fixed_values, self.fixed_polys, self.fixed_cosets, self.permutations, self.permutation_polys, self.permutation_cosets):
+            yield struct.pack(">I", len(ps)) + struct.pack(">%dI" % len(ps), *[len(p) for p in ps])
+            for p in ps:
+                yield from poly(p)
+
+    def to_bytes(self) -> bytes:
+        """ProvingKey::write(.., SerdeFormat::RawBytes): the inverse of `read`."""
+        return b"".join(self._chunks())
+
+    def write(self, path: str):
+        """to_bytes() streamed to a file, one column at a time."""
+        with open(path, "wb") as f:
+            for c in self._chunks():
+                f.write(c)
+
+    SECTIONS = ("l0", "l_last", "l_active_row", "fixed_values", "fixed_polys", "fixed_cosets", "permutations", "permutation_polys",
+                "permutation_cosets")
+
+    @staticmethod
+    def layout(buf, num_permutation_columns: int, num_selectors: int, ext_k: int) -> dict:
+        """Walks the section headers of a RawBytes key in `buf` (bytes, or a memory map) reading only the u32 counts and lengths, never
+        a column's elements -> {"k", "vk_len", section: [byte offset of each column's first element]} for the SECTIONS (the three
+        l-vectors as one-column lists).  Raises B200Error for a version other than 3, a column count or length that does not fit the
+        given counts (the vk's fixed columns, num_permutation_columns; 2^k elements for values and polys, 2^ext_k for cosets and
+        l-vectors, in the length table too), a truncated file and trailing bytes."""
+        size = len(buf)
+        if size < 7:
+            raise nat.B200Error("pk layout: %d bytes, no vk header" % size)
+        ver, k = int(buf[0]), int(buf[1])
+        if ver != 3:
+            raise nat.B200Error("pk layout: unsupported key version %d" % ver)
+        if not 1 <= k <= ext_k <= F.FR_S:
+            raise nat.B200Error("pk layout: need 1 <= k = %d <= ext_k = %d <= %d" % (k, ext_k, F.FR_S))
+        (nf,) = struct.unpack_from("<I", buf, 3)
+        n, N = 1 << k, 1 << ext_k
+        off = 7 + 64 * nf + 64 * num_permutation_columns + num_selectors * (n // 8)
+        out = {"k": k, "vk_len": off}
+
+        def u32(at):
+            if at + 4 > size:
+                raise nat.B200Error("pk layout: truncated at byte %d of %d" % (at, size))
+            return struct.unpack_from(">I", buf, at)[0]
+
+        def poly(name, at, length):
+            got = u32(at)
+            if got != length:
+                raise nat.B200Error("pk layout: %s has a column of length %d, expected %d" % (name, got, length))
+            if at + 4 + 32 * length > size:
+                raise nat.B200Error("pk layout: %s is truncated at byte %d of %d" % (name, at, size))
+            return at + 4, at + 4 + 32 * length
+
+        for name in ProvingKey.SECTIONS:
+            cols, length = (nf if name.startswith("fixed") else num_permutation_columns), (n if name.endswith(("values", "polys", "permutations")) else N)
+            if name.startswith("l"):
+                start, off = poly(name, off, N)
+                out[name] = [start]
+                continue
+            cnt = u32(off)
+            if cnt != cols:
+                raise nat.B200Error("pk layout: %s has %d columns, expected %d" % (name, cnt, cols))
+            for j in range(cnt):
+                if u32(off + 4 + 4 * j) != length:
+                    raise nat.B200Error("pk layout: %s's length table gives column %d length %d, expected %d" % (name, j, u32(off + 4 + 4 * j), length))
+            off += 4 + 4 * cnt
+            out[name] = []
+            for _ in range(cnt):
+                start, off = poly(name, off, length)
+                out[name].append(start)
+        if off != size:
+            raise nat.B200Error("pk layout: %d trailing bytes (wrong column counts?)" % (size - off))
+        return out
+
     def keygen_pk_polys(self, j: int, blinding_factors: int):
         """Recompute on the device what keygen_pk derives (create_keys, /root/reference/src/pfsys/mod.rs:376-400):
         fixed_polys / cosets, permutation polys / cosets, l0 / l_last / l_active_row.  Returns a dict of lists."""
