@@ -413,19 +413,21 @@ def _verifier_accumulate(keys: Keys, proof: bytes, instances=()):
     except KeyError:
         return None
     expected_h = numerator * pow(xn - 1, -1, R) % R
-    # openings as (list of (scalar, point)) commitments, point, eval — same order as the prover's queries
-    qs = [([(1, adv_c[c])], rot_pt(rot), v) for (c, rot), v in zip(cs.advice_queries, adv_e)]
+    # openings as (source, list of (scalar, point)) commitments, point, eval — same order as the prover's queries.  `source` names the
+    # polynomial an opening belongs to: two columns with equal contents (two all-zero selectors) have equal commitments, yet the prover
+    # opens them as two polynomials, so the rotation sets below must not merge them
+    qs = [(("advice", c), [(1, adv_c[c])], rot_pt(rot), v) for (c, rot), v in zip(cs.advice_queries, adv_e)]
     for i in range(cs.num_z):
-        qs += [([(1, z_c[i])], x, z_e[i][0]), ([(1, z_c[i])], rot_pt(1), z_e[i][1])]
+        qs += [(("z", i), [(1, z_c[i])], x, z_e[i][0]), (("z", i), [(1, z_c[i])], rot_pt(1), z_e[i][1])]
     for i in reversed(range(cs.num_z - 1)):
-        qs.append(([(1, z_c[i])], rot_pt(last_rot), z_e[i][2]))
+        qs.append((("z", i), [(1, z_c[i])], rot_pt(last_rot), z_e[i][2]))
     for i in range(len(cs.lookups)):
-        qs += [([(1, phi_c[i])], x, lk_e[i][0]), ([(1, phi_c[i])], rot_pt(1), lk_e[i][1]), ([(1, m_c[i])], x, lk_e[i][2])]
+        qs += [(("phi", i), [(1, phi_c[i])], x, lk_e[i][0]), (("phi", i), [(1, phi_c[i])], rot_pt(1), lk_e[i][1]), (("m", i), [(1, m_c[i])], x, lk_e[i][2])]
     fx = [_jac_to_xy(c) for c in keys.fixed_commitments]
     sg = [_jac_to_xy(c) for c in keys.sigma_commitments]
-    qs += [([(1, fx[c - na])], rot_pt(rot), v) for (c, rot), v in zip(cs.fixed_queries, fix_e)]
-    qs += [([(1, sg[i])], x, sig_e[i]) for i in range(len(sg))]
-    qs += [([(pow(xn, i, R), h_c[i]) for i in range(len(h_c))], x, expected_h), ([(1, rand_c)], x, rand_e)]
+    qs += [(("fixed", c), [(1, fx[c - na])], rot_pt(rot), v) for (c, rot), v in zip(cs.fixed_queries, fix_e)]
+    qs += [(("sigma", i), [(1, sg[i])], x, sig_e[i]) for i in range(len(sg))]
+    qs += [(("h",), [(pow(xn, i, R), h_c[i]) for i in range(len(h_c))], x, expected_h), (("random",), [(1, rand_c)], x, rand_e)]
     try:
         y2, v = tr.squeeze_challenge(), tr.squeeze_challenge()
         h1 = tr.read_ec_point()
@@ -435,10 +437,9 @@ def _verifier_accumulate(keys: Keys, proof: bytes, instances=()):
         return None
     if tr.pos != len(proof):
         return None
-    # rotation sets keyed by the commitment's identity (same grouping rule as the prover: first appearance order)
+    # rotation sets keyed by the opened polynomial's source, not by the commitment's value (the prover's grouping rule, first appearance order)
     by_commit, order = {}, []
-    for comm, pt, val in qs:
-        key = tuple((sc, p) for sc, p in comm)
+    for key, comm, pt, val in qs:
         if key not in by_commit:
             by_commit[key] = (comm, [], [])
             order.append(key)
