@@ -1,11 +1,10 @@
-"""ctypes binding of libezkl_b200.so (the C ABI in include/ezkl_b200.h, include/ezkl_b200_resident.h, include/ezkl_b200_keygen.h,
-include/ezkl_b200_srs.h and include/ezkl_b200_pk.h).
+"""ctypes binding of libezkl_b200.so (the C ABI in include/ezkl_b200.h).
 
 There is no fallback: if the shared library is missing, or b200_init finds no sm_90 device, the error is raised to the
 caller.  Arrays are numpy uint64 in the wire format (Fr -> [...,4], G1Affine -> [...,8], G1 Jacobian -> [...,12],
 XYZZ -> [...,16]); device-resident entry points take raw device pointers (ints), e.g. torch ``tensor.data_ptr()``.
 
-Every b200_* function gets its argtypes / restype from the prototypes of its C headers when the library is loaded, so ctypes
+Every b200_* function gets its argtypes / restype from the prototypes of its C header when the library is loaded, so ctypes
 converts Python ints at the declared width and rejects a call with the wrong number of arguments before it reaches C.
 """
 from __future__ import annotations
@@ -19,10 +18,6 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libezkl_b200.so")
 HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200.h")
-RESIDENT_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_resident.h")     # entry points for device-resident callers
-KEYGEN_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_keygen.h")         # key-generation entry points
-SRS_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_srs.h")               # SRS file -> registered base tables
-PK_HEADER = os.path.join(os.path.dirname(_HERE), "include", "ezkl_b200_pk.h")                 # proving-key file -> device columns
 DBG_LIB_PATH = os.path.join(_HERE, "libezkl_b200_dbg.so")
 DBG_HEADER = os.path.join(_HERE, "csrc", "debug.h")
 
@@ -63,16 +58,15 @@ def declarations(header: str) -> dict:
     return out
 
 
-def _load(path: str, headers, build_hint: str):
+def _load(path: str, header: str, build_hint: str):
     if not os.path.exists(path):
         raise B200Error("%s is not built: run %s (there is no CPU fallback)" % (os.path.basename(path), build_hint))
     lib = C.CDLL(path)
-    for header in headers:
-        for name, (argtypes, restype) in declarations(header).items():
-            fn = getattr(lib, name, None)
-            if fn is None:
-                raise B200Error("%s does not export %s, which %s declares: rebuild it" % (os.path.basename(path), name, header))
-            fn.argtypes, fn.restype = argtypes, restype
+    for name, (argtypes, restype) in declarations(header).items():
+        fn = getattr(lib, name, None)
+        if fn is None:
+            raise B200Error("%s does not export %s, which %s declares: rebuild it" % (os.path.basename(path), name, header))
+        fn.argtypes, fn.restype = argtypes, restype
     return lib
 
 
@@ -84,7 +78,7 @@ _inited = False
 def lib():
     global _lib
     if _lib is None:
-        _lib = _load(LIB_PATH, (HEADER, RESIDENT_HEADER, KEYGEN_HEADER, SRS_HEADER, PK_HEADER), "`python -c 'import __graft_entry__ as g; g.build()'` or `make -C ezkl_b200/csrc`")
+        _lib = _load(LIB_PATH, HEADER, "`python -c 'import __graft_entry__ as g; g.build()'` or `make -C ezkl_b200/csrc`")
     return _lib
 
 
@@ -92,7 +86,7 @@ def dbg_lib():
     """Test-only companion library (b200_debug_*: per-layer self tests and microbenchmarks).  The product never loads it."""
     global _dbg
     if _dbg is None:
-        _dbg = _load(DBG_LIB_PATH, (DBG_HEADER,), "`make -C ezkl_b200/csrc`")
+        _dbg = _load(DBG_LIB_PATH, DBG_HEADER, "`make -C ezkl_b200/csrc`")
     return _dbg
 
 

@@ -16,10 +16,6 @@
 #include <vector>
 
 #include "../../include/ezkl_b200.h"
-#include "../../include/ezkl_b200_keygen.h"
-#include "../../include/ezkl_b200_pk.h"
-#include "../../include/ezkl_b200_resident.h"
-#include "../../include/ezkl_b200_srs.h"
 #include "msm.cuh"
 #include "ntt.cuh"
 #include "poly.cuh"
@@ -192,6 +188,12 @@ static size_t call_budget() {
     const size_t lo = (size_t)256 << 20, hi = (size_t)12 << 30;
     return per < lo ? lo : (per > hi ? hi : per);
 }
+// how many columns of item_bytes each one call may stage: at least one, then at most max_items
+static size_t group_size(size_t item_bytes, size_t max_items) {
+    size_t g = call_budget() / item_bytes;
+    if (g < 1) g = 1;
+    return g < max_items ? g : max_items;
+}
 // host Fr values arrive with 8-byte alignment (Rust / C callers); Fr is alignas(16), so always copy bytewise
 static inline Fr as_fr(const b200_fr* p) { Fr r; memcpy(&r, p, sizeof r); return r; }
 
@@ -303,6 +305,12 @@ static int ring_upload(Ctx* c, void* d_dst, const void* h_src, size_t bytes, cud
 }
 static int h2d_one(Ctx* c, void* d_dst, const void* h_src, size_t bytes, cudaStream_t st) { HostSeg s{(uint8_t*)const_cast<void*>(h_src), bytes}; return h2d_segments(c, d_dst, &s, 1, st); }
 static int d2h_one(Ctx* c, void* h_dst, const void* d_src, size_t bytes, cudaStream_t st) { HostSeg s{(uint8_t*)h_dst, bytes}; return d2h_segments(c, d_src, &s, 1, st); }
+// a few bytes of device results (a counter, a check word) -> host memory, after the work queued before them on `st`
+static int read_back(void* h_dst, const void* d_src, size_t bytes, cudaStream_t st) {
+    B200_CUDA(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
 
 // XYZZ (host) -> normalised Jacobian, one shared inversion (Montgomery's trick over zz*zzz)
 static void normalize_host(const G1Xyzz* pts, size_t n, b200_g1_jac* out) {
@@ -401,6 +409,10 @@ static int ntt_scales(int pre_mode, const b200_fr* pre, int post_mode, const b20
     for (int i = 0; i < post_mode; ++i) b->c[i] = as_fr(post + i);
     return 0;
 }
+// the zeta coset of coeff_to_extended: coefficient i is pre-scaled by zeta^(i mod 3)
+static NttScale coset_pre(const Fr& zeta) { NttScale s; s.mode = 3; s.c[0] = fp_one<FrTag>(); s.c[1] = zeta; s.c[2] = zeta * zeta; return s; }
+// its undoing in extended_to_coeff, with the inverse transform's divisor d: element i is post-scaled by d zeta^-(i mod 3), zeta^-1 = zeta^2
+static NttScale coset_post(const Fr& d, const Fr& zeta) { NttScale s; s.mode = 3; s.c[0] = d; s.c[1] = d * (zeta * zeta); s.c[2] = d * zeta; return s; }
 
 // ---- device workers: one host thread per extra device, so that the host-pointer entry points of a multi-device process drive
 //      every PCIe link and every GPU at once (a single thread staging pageable memory serialises on its own copies) ------------
@@ -454,10 +466,8 @@ static int msm_dev_on(Ctx* c, cudaStream_t st, const BaseSet* bs, const Fr* sc, 
     const MsmTable* t = bs->t[c->slot];
     B200_CHECK(t, -1, "msm: the bases have no replica on device slot %d", c->slot);
     const size_t per_col = msm_workspace_per_column(*t, n);
-    size_t sub = call_budget() / (per_col ? per_col : 1);
-    if (sub < 1) sub = 1;
-    if (sub > 4096) sub = 4096;
-    if (sub > (size_t)(65535 / t->s)) sub = 65535 / t->s;          // a reduced table reduces batch * s bucket sets in one grid
+    const size_t max_grid = (size_t)(65535 / t->s);                 // a reduced table reduces batch * s bucket sets in one grid
+    const size_t sub = group_size(per_col ? per_col : 1, max_grid < 4096 ? max_grid : 4096);
     for (size_t b0 = 0; b0 < batch; b0 += sub) {
         const size_t nb = batch - b0 < sub ? batch - b0 : sub;
         if (int rc = msm_run(*t, sc + b0 * stride, n, stride, (int)nb, out + b0, c->msm_ws, st, base_off)) return rc;
@@ -469,9 +479,7 @@ static int msm_host_on(Ctx* c, const BaseSet* bs, const b200_fr* const* cols, si
     if (count == 0) return 0;
     if (n == 0) { memset(h_out, 0, sizeof(G1Xyzz) * count); return 0; }
     DevGuard dg(c);
-    size_t sub = call_budget() / (sizeof(Fr) * n * 2);
-    if (sub < 1) sub = 1;
-    if (sub > count) sub = count;
+    const size_t sub = group_size(sizeof(Fr) * n * 2, count);
     if (c->stage_a.ensure(sizeof(Fr) * n * sub) || c->small.ensure(sizeof(G1Xyzz) * count)) return -2;
     StreamScope ss(c, nullptr);
     for (size_t b0 = 0; b0 < count; b0 += sub) {
@@ -951,9 +959,7 @@ static int ntt_host_on(Ctx* c, const b200_fr* const* src, b200_fr* const* dst, s
     if (batch == 0) return 0;
     DevGuard dg(c);
     const size_t N = (size_t)1 << log_n;
-    size_t sub = call_budget() / (sizeof(Fr) * N * 3);
-    if (sub < 1) sub = 1;
-    if (sub > batch) sub = batch;
+    const size_t sub = group_size(sizeof(Fr) * N * 3, batch);
     if (c->stage_a.ensure(sizeof(Fr) * n_in * sub) || c->stage_b.ensure(sizeof(Fr) * N * sub) || c->stage_c.ensure(sizeof(Fr) * N * sub)) return -2;
     StreamScope ss(c, nullptr);
     for (size_t b0 = 0; b0 < batch; b0 += sub) {
@@ -1034,9 +1040,8 @@ int b200_ifft(b200_fr* a, uint32_t log_n, const b200_fr* omega_inv, const b200_f
 }
 int b200_coeff_to_extended_batch(const b200_fr* const* coeffs, size_t batch, size_t n_coeffs, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta, b200_fr* const* out) {
     B200_CHECK(coeffs && out && ext_omega && zeta, -1, "coeff_to_extended: null pointer");
-    NttScale pre, none;
-    pre.mode = 3; pre.c[0] = fp_one<FrTag>(); pre.c[1] = as_fr(zeta); pre.c[2] = as_fr(zeta) * as_fr(zeta);
-    return ntt_host(coeffs, out, batch, n_coeffs, ext_k, as_fr(ext_omega), pre, none);
+    NttScale none;
+    return ntt_host(coeffs, out, batch, n_coeffs, ext_k, as_fr(ext_omega), coset_pre(as_fr(zeta)), none);
 }
 int b200_coeff_to_extended(const b200_fr* coeffs, size_t n_coeffs, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta, b200_fr* out) {
     const b200_fr* s[1] = {coeffs}; b200_fr* d[1] = {out};
@@ -1044,11 +1049,9 @@ int b200_coeff_to_extended(const b200_fr* coeffs, size_t n_coeffs, uint32_t ext_
 }
 int b200_extended_to_coeff(b200_fr* a, uint32_t ext_k, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, const b200_fr* zeta) {
     B200_CHECK(a && ext_omega_inv && ext_ifft_divisor && zeta, -1, "extended_to_coeff: null pointer");
-    NttScale none, post;
-    const Fr z = as_fr(zeta), z2 = z * z, d = as_fr(ext_ifft_divisor);
-    post.mode = 3; post.c[0] = d; post.c[1] = d * z2; post.c[2] = d * z;     // zeta^-1 = zeta^2
+    NttScale none;
     b200_fr* p[1] = {a};
-    return ntt_host(p, p, 1, (size_t)1 << (ext_k <= 28 ? ext_k : 0), ext_k, as_fr(ext_omega_inv), none, post);
+    return ntt_host(p, p, 1, (size_t)1 << (ext_k <= 28 ? ext_k : 0), ext_k, as_fr(ext_omega_inv), none, coset_post(as_fr(ext_ifft_divisor), as_fr(zeta)));
 }
 
 // ---- polynomial ops --------------------------------------------------------------------------------------------
@@ -1227,8 +1230,7 @@ static int lookup_multiplicities_on(Ctx* c, cudaStream_t st, const void* d_table
                                            reinterpret_cast<Fr*>(d_m), c->msm_ws.misc, c->ring, &d_missing, st)) return rc;
     if (missing) {
         unsigned long long h = 0;
-        B200_CUDA(cudaMemcpyAsync(&h, d_missing, sizeof h, cudaMemcpyDeviceToHost, st));
-        B200_CUDA(cudaStreamSynchronize(st));
+        if (int rc = read_back(&h, d_missing, sizeof h, st)) return rc;
         *missing = h;
     }
     return 0;
@@ -1259,7 +1261,7 @@ int b200_lookup_multiplicities(const b200_fr* table, size_t n_table, const b200_
     return 0;
 }
 
-// ---- permutation keygen (include/ezkl_b200_keygen.h) ------------------------------------------------------------------------
+// ---- permutation keygen ------------------------------------------------------------------------------------------------------------
 // n_map_columns mapping columns at d_map -> sigma columns at d_out (stride out_stride); a cell is valid when its column is < n_columns and its
 // row < 2^k.  The host-pointer entry point calls this once per column group, with n_columns = every column of the key.
 static int perm_sigmas_on(Ctx* c, cudaStream_t st, const void* d_map, size_t n_map_columns, size_t n_columns, uint32_t k, const b200_fr* omega, const b200_fr* delta,
@@ -1292,8 +1294,7 @@ int b200_permutation_sigmas_dev(const void* d_mapping, size_t n_columns, uint32_
     if (int rc = perm_sigmas_on(c, ss.st, d_mapping, n_columns, n_columns, k, omega, delta, d_out, out_stride, d_inv)) return rc;
     if (invalid) {
         unsigned long long h = 0;
-        B200_CUDA(cudaMemcpyAsync(&h, d_inv, sizeof h, cudaMemcpyDeviceToHost, ss.st));
-        B200_CUDA(cudaStreamSynchronize(ss.st));
+        if (int rc = read_back(&h, d_inv, sizeof h, ss.st)) return rc;
         *invalid = h;
     }
     return 0;
@@ -1317,9 +1318,7 @@ static int perm_sigmas_host_on(Ctx* c, const uint32_t* mapping, const size_t* co
     if (count == 0) return 0;
     DevGuard dg(c);
     const size_t n = (size_t)1 << k, map_bytes = 2 * sizeof(uint32_t) * n, col_bytes = sizeof(Fr) * n;
-    size_t sub = call_budget() / (map_bytes + col_bytes);
-    if (sub < 1) sub = 1;
-    if (sub > count) sub = count;
+    const size_t sub = group_size(map_bytes + col_bytes, count);
     if (c->stage_a.ensure(map_bytes * sub) || c->stage_b.ensure(col_bytes * sub)) return -2;
     StreamScope ss(c, nullptr);
     for (size_t b0 = 0; b0 < count; b0 += sub) {
@@ -1430,6 +1429,7 @@ static int evaluate_h_parts_on(Ctx* c, cudaStream_t st, const Fr* const* cols, c
     const uint32_t lo_bits = (ext_k + 1) / 2;
     const Fr* d_tab = nullptr;
     const FoldCol* d_fold = nullptr;
+    NttScale zeta_cycle = coset_pre(zeta), none;
     if (p > 0 && !fold.empty()) {
         const size_t n_lo = (size_t)1 << lo_bits, n_hi = N >> lo_bits, n_tab = 3 + n_lo + n_hi;
         // [1, zeta, zeta^2 | w_N^e, e < n_lo | w_N^(e n_lo), e < n_hi | the fold table], staged once for every part
@@ -1437,7 +1437,7 @@ static int evaluate_h_parts_on(Ctx* c, cudaStream_t st, const Fr* const* cols, c
         if (c->small.ensure(tab_bytes + fold_bytes)) return -2;
         std::vector<uint8_t> blob(tab_bytes + fold_bytes);
         Fr* tab = reinterpret_cast<Fr*>(blob.data());
-        tab[0] = fp_one<FrTag>(); tab[1] = zeta; tab[2] = zeta * zeta;
+        for (int i = 0; i < 3; ++i) tab[i] = zeta_cycle.c[i];
         omega_power_table(tab + 3, lo_bits, ext_k, ext_omega);
         memcpy(blob.data() + tab_bytes, fold.data(), fold_bytes);
         if (int rc = ring_upload(c, c->small.p, blob.data(), blob.size(), st)) return rc;
@@ -1449,8 +1449,6 @@ static int evaluate_h_parts_on(Ctx* c, cudaStream_t st, const Fr* const* cols, c
     std::vector<const void*> ptrs(n_columns);
     std::vector<uint32_t> shifts(n_columns, 0);
     for (size_t i = 0, j = 0; i < n_columns; ++i) if (lengths[i] < N) ptrs[i] = parts + m * j++;
-    NttScale zeta_cycle, none;
-    zeta_cycle.mode = 3; zeta_cycle.c[0] = fp_one<FrTag>(); zeta_cycle.c[1] = zeta; zeta_cycle.c[2] = zeta * zeta;
     for (size_t part = 0; part < P; ++part) {
         if (p == 0) {
             for (size_t j = 0; j < fold.size(); ++j) {
@@ -1479,10 +1477,8 @@ static int evaluate_h_finish(Ctx* c, cudaStream_t st, Fr* h, Fr* scratch, uint32
                              const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor) {
     const size_t N = (size_t)1 << ext_k;
     if (int rc = scale_cycle_on(c, st, h, N, t_evaluations, t_period)) return rc;
-    const Fr z = as_fr(zeta), z2 = z * z, d = as_fr(ext_ifft_divisor);
-    NttScale none, post;
-    post.mode = 3; post.c[0] = d; post.c[1] = d * z2; post.c[2] = d * z;
-    return ntt_call(c, st, h, N, N, scratch, h, N, ext_k, as_fr(ext_omega_inv), none, post, 1);
+    NttScale none;
+    return ntt_call(c, st, h, N, N, scratch, h, N, ext_k, as_fr(ext_omega_inv), none, coset_post(as_fr(ext_ifft_divisor), as_fr(zeta)), 1);
 }
 
 // evaluate_h at its natural boundary: the CPU evaluator receives coefficient-form polynomials and builds their cosets itself
@@ -1538,7 +1534,7 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
     return d2h_one(c, out, h, sizeof(Fr) * N, ss.st);
 }
 
-// evaluate_h on device-resident columns (include/ezkl_b200_resident.h): always by parts, on the caller's columns where they are
+// evaluate_h on device-resident columns: always by parts, on the caller's columns where they are
 int b200_evaluate_h_dev(const void* const* d_polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k, const b200_fr* ext_omega, const b200_fr* zeta,
                         const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr,
                         const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, void* d_out, void* stream) {
@@ -1565,7 +1561,7 @@ int b200_evaluate_h_dev(const void* const* d_polys, const size_t* lengths, size_
     return evaluate_h_finish(c, ss.st, h, c->stage_b.as<Fr>(), ext_k, zeta, t_evaluations, t_period, ext_omega_inv, ext_ifft_divisor);
 }
 
-// ---- SRS (include/ezkl_b200_srs.h) ------------------------------------------------------------------------------------------------
+// ---- SRS --------------------------------------------------------------------------------------------------------------------------
 // Fr's 2^28-th root of unity (halo2curves Fr::ROOT_OF_UNITY = 7^((r - 1) / 2^28)) in Montgomery form
 static Fr fr_root_of_unity() {
     Fr w;
@@ -1633,7 +1629,7 @@ int b200_srs_register(const b200_g1_affine* g, const b200_g1_affine* g_lagrange,
     return srs_register_on(c, ss.st, g, g_lagrange, k, window_bits, max_table_bytes, g_handle, g_lagrange_handle);
 }
 
-// ---- proving key (include/ezkl_b200_pk.h) -----------------------------------------------------------------------------------------
+// ---- proving key ------------------------------------------------------------------------------------------------------------------
 // Fr::ZETA (halo2curves), the cube root of unity that coeff_to_extended distributes as [1, zeta, zeta^2], in Montgomery form
 static Fr fr_zeta() {
     Fr z;
@@ -1661,25 +1657,21 @@ static int pk_load_on(Ctx* c, cudaStream_t st, const void* const* cols, size_t n
         if (int rc = fr_validate_run(values + j * stride, n, j, d_first, st)) return rc;
     }
     unsigned long long first = ~0ull;
-    B200_CUDA(cudaMemcpyAsync(&first, d_first, sizeof first, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
+    if (int rc = read_back(&first, d_first, sizeof first, st)) return rc;
     if (first != ~0ull) {
         const size_t col = (size_t)(first >> 32), row = (size_t)(first & 0xffffffffu);
         set_error("pk_load: %s[%zu][%zu] is not below r", col < n_fixed ? "fixed_values" : "permutations", col < n_fixed ? col : col - n_fixed, row);
         return -1;
     }
-    const size_t budget = call_budget();
-    size_t g = budget / (sizeof(Fr) * n), s = budget / (sizeof(Fr) * N);
-    g = g < 1 ? 1 : (g > n_cols ? n_cols : (g > 65535 ? 65535 : g));
-    s = s < 1 ? 1 : (s > 3 ? 3 : s);
+    const size_t g = group_size(sizeof(Fr) * n, n_cols < 65535 ? n_cols : 65535), s = group_size(sizeof(Fr) * N, 3);
     const size_t tmp_elems = g * n > s * N ? g * n : s * N;
     if (c->stage_a.ensure(sizeof(Fr) * 3 * n) || c->stage_b.ensure(sizeof(Fr) * tmp_elems)) return -2;
     Fr* coef = c->stage_a.as<Fr>();
     Fr* tmp = c->stage_b.as<Fr>();
-    const Fr w_inv = fp_inv(fr_omega(k)), zeta = fr_zeta();
-    NttScale none, div_n, zeta_cycle;
+    const Fr w_inv = fp_inv(fr_omega(k));
+    const NttScale zeta_cycle = coset_pre(fr_zeta());
+    NttScale none, div_n;
     div_n.mode = 1; div_n.c[0] = fr_inv_u64(n);
-    zeta_cycle.mode = 3; zeta_cycle.c[0] = fp_one<FrTag>(); zeta_cycle.c[1] = zeta; zeta_cycle.c[2] = zeta * zeta;
     for (size_t j0 = 0; j0 < n_cols; j0 += g) {
         const int nb = (int)(n_cols - j0 < g ? n_cols - j0 : g);
         if (int rc = ntt_call(c, st, values + j0 * stride, stride, n, tmp, polys + j0 * stride, stride, k, w_inv, none, div_n, nb)) return rc;

@@ -7,7 +7,7 @@
 // Radix-2 decimation-in-time on XYZZ points in global memory, one kernel per stage; each butterfly multiplies its odd input by
 // a 254-bit twiddle with a 4-bit fixed-window ladder (the table of 1..15 multiples lives in the thread's local memory).
 // Bound: n/2 * log n * ~3000 field multiplications — pure multiply issue, like everything else here.
-// Also here: k_g1_validate, the point check of an SRS vector read from a file (b200_srs_register, include/ezkl_b200_srs.h).
+// Also here: k_g1_validate, the point check of an SRS vector read from a file (b200_srs_register, include/ezkl_b200.h).
 #include "msm.cuh"
 
 namespace b200 {

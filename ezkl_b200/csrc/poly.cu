@@ -139,7 +139,7 @@ int perm_sigmas_run(const uint32_t* d_map, size_t n_columns, uint32_t k, const F
     return 0;
 }
 
-// ---- proving-key load (b200_pk_load, include/ezkl_b200_pk.h) ----------------------------------------------------------------
+// ---- proving-key load (b200_pk_load, include/ezkl_b200.h) --------------------------------------------------------------------
 // The check of one key column as halo2curves' Fr::from_raw_bytes makes it: one thread per element, 32 B read and one limb comparison,
 // so HBM-bound.  Rows of a warp are consecutive, so its lowest failing lane is its lowest failing row: one atomicMin per warp at most,
 // on (column << 32 | row), which keeps the lowest (column, row) of the call.

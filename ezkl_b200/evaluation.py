@@ -311,7 +311,7 @@ def evaluate_h_from_polys(program: QuotientProgram, polys, domain, finish: bool 
 def evaluate_h_from_polys_device(program: QuotientProgram, polys, domain, finish: bool = False, out=None):
     """b200_evaluate_h_dev: evaluate_h_from_polys on device-resident columns.  polys = contiguous torch int64 CUDA tensors [len, 4], each in
     coefficient form (len < 2^ext_k) or extended (len == 2^ext_k); they may be views of one allocation.  Evaluated one n-point coset part at
-    a time with the extended columns read in place (include/ezkl_b200_resident.h); the same bytes as evaluate_h_from_polys.  Enqueued on
+    a time with the extended columns read in place (include/ezkl_b200.h); the same bytes as evaluate_h_from_polys.  Enqueued on
     torch's current stream; returns `out` ([2^ext_k, 4], allocated when None)."""
     import torch
     from .device import _stream

@@ -217,6 +217,142 @@ int b200_evaluate_h(const b200_fr* const* polys, const size_t* lengths, size_t n
                     const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants, const b200_instr* program, size_t n_instr,
                     const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor, b200_fr* out);
 
+/* ---- quotient from device-resident columns: b200_evaluate_h for callers that keep a proof's columns on the device -----------------
+ * (INTEGRATION.md §2b): the witness, the key's polynomials and every column derived from them stay in device memory for the whole proof,
+ * and each stage is handed device pointers.  The device-pointer twin of b200_evaluate_h, with the same semantics and the same result bytes:
+ *   - column i of the program is coeff_to_extended(d_polys[i]) when lengths[i] < 2^ext_k (coefficient form: the advice, lookup and
+ *     permutation polynomials, ProvingKey.fixed_polys / permutation.polys), and d_polys[i] itself when lengths[i] == 2^ext_k (an
+ *     extended column: the key's l0 / l_last / l_active_row cosets, a running partial sum);
+ *   - the program encoding is that of b200_quotient_eval;
+ *   - t_evaluations == NULL: d_out = the numerator on the extended domain (2^ext_k elements).  Otherwise d_out = the quotient's 2^ext_k
+ *     coefficients, extended_to_coeff(numerator * t_evaluations[i mod t_period]), which needs t_period in 1 ... 1024, ext_omega_inv
+ *     and ext_ifft_divisor;
+ *   - the result equals b200_evaluate_h's on the same columns, byte for byte, whatever that call's scratch budget selects.
+ * Pointers and streams: d_polys[i] and d_out are device pointers; every other pointer is host memory, read during the call.  The call
+ * runs on the device that owns d_out, is enqueued on `stream` (NULL = the calling thread's library stream) and does not synchronise.
+ * Columns are read-only and may overlap each other (views of one allocation); d_out must not overlap any column [d_polys[i],
+ * d_polys[i] + 32 * lengths[i]).
+ * One path: the numerator is evaluated one n-point coset part at a time, n = 2^k, for the d = 2^(ext_k - k) parts c < d (the extended
+ * indices c + d i; one part when k == ext_k).  Per part, every coefficient column is folded and transformed into its n-point part;
+ * extended columns are read where they are, every d-th element from d_polys[i] + c, never copied; the interpreter stores row i at
+ * index c + d i of d_out.  The finishing step then runs in place in d_out.  The per-call scratch budget (B200_WS_BUDGET_MB) selects
+ * nothing here, because the caller's columns are already resident.
+ * Device scratch held by the calling thread: n_coeff * 2^k * 32 B (the coefficient columns' parts, n_coeff = the number of columns
+ * with lengths[i] < 2^ext_k) + 2^ext_k * 32 B (transform scratch) + the power table ((3 + 2^ceil(ext_k/2) + 2^floor(ext_k/2)) * 32 B)
+ * and 16 B per coefficient column; each buffer is allocated with 1/8 headroom, and the transform plans of sizes 2^k and 2^ext_k come on
+ * top.  At k = 22, ext_k = 25 with 129 coefficient columns that is 17.1 GiB stated and 20.4 GiB held after a finished call (H100 80GB
+ * HBM3, 700 W; DESIGN.md §4.4).
+ * Argument errors return -1, with a message in b200_last_error(), and write nothing to d_out: a null pointer (d_polys and lengths may be
+ * NULL when n_columns == 0), a length of 0 or above 2^ext_k, k == 0, k > ext_k or ext_k > 28, finishing without its constants or with
+ * t_period outside 1 ... 1024, d_out overlapping a column, and every program check of b200_quotient_eval_dev. */
+int b200_evaluate_h_dev(const void* const* d_polys, const size_t* lengths, size_t n_columns, uint32_t k, uint32_t ext_k,
+                        const b200_fr* ext_omega, const b200_fr* zeta,
+                        const b200_col_ref* loads, size_t n_loads, const b200_fr* constants, size_t n_constants,
+                        const b200_instr* program, size_t n_instr,
+                        const b200_fr* t_evaluations, uint32_t t_period, const b200_fr* ext_omega_inv, const b200_fr* ext_ifft_divisor,
+                        void* d_out, void* stream);
+
+/* ---- permutation keygen: the sigma columns (halo2 plonk/permutation/keygen.rs, Assembly::build_vk / build_pk) -------------------
+ * A step of create_keys (keygen_vk / keygen_pk) that is not also a step of create_proof.
+ * The mapping is the Assembly's after every copy constraint has been merged into its cycles: n_columns * 2^k pairs of uint32
+ * (column, row), column-major, so cell (column j, row i) sits at mapping[2 * (j * 2^k + i)] (its column) and
+ * mapping[2 * (j * 2^k + i) + 1] (its row).  The shim flattens halo2's `mapping: Vec<Vec<(usize, usize)>>` into this layout.
+ * Sigma column j, row i = delta^c * omega^r where (c, r) is cell (j, i)'s entry: Fr in Montgomery form, fully reduced, so the bytes are
+ * those of build_pk's `permutations` (halo2 computes them as a table of delta^j * omega^i followed by a gather).  omega = the domain's
+ * n-th root of unity, delta = Fr::DELTA.  The library does not check that the mapping is a permutation (halo2 does not either); it only
+ * needs every column < n_columns and every row < 2^k.
+ * Both entry points: -1 for k > 28, and for a null pointer when n_columns > 0; 0 with no work when n_columns == 0.
+ *
+ * Host pointers: out[j] receives sigma column j (2^k elements).  Every cell is checked on the host before any device work: a cell
+ * outside n_columns x 2^k returns -1 and writes nothing.  The mapping and the results are staged in column groups bounded by the
+ * per-call scratch budget (B200_WS_BUDGET_MB, else derived from B200_WS_TOTAL_MB), which holds a group's 40 B per cell (8 B of mapping
+ * and 32 B of result), so k = 26 and beyond need no more than one column at a time.  In a multi-device process the columns are dealt
+ * over the devices, each staging its own columns over its own PCIe link.
+ * Device pointers: sigma column j at d_out + 32 * j * out_stride bytes (out_stride >= 2^k elements, else -1); d_out must not overlap
+ * d_mapping.  A cell outside n_columns x 2^k is written as zero; when `invalid` is non-NULL it receives the number of such cells and
+ * the call synchronises its stream, otherwise the call only enqueues.  Runs on the device that owns d_out.
+ * Device memory held beyond the caller's buffers: the table [delta^c, c < n_columns | omega^e, e < 2^ceil(k/2) | omega^(e 2^ceil(k/2)),
+ * e < 2^floor(k/2)], 32 B per entry, in the thread's parameter ring (a slot up to 256 KiB, a reused device buffer above), 8 B for the
+ * counter of invalid cells, and for the host-pointer form the staging of one column group. */
+int b200_permutation_sigmas(const uint32_t* mapping, size_t n_columns, uint32_t k, const b200_fr* omega, const b200_fr* delta, b200_fr* const* out);
+int b200_permutation_sigmas_dev(const void* d_mapping, size_t n_columns, uint32_t k, const b200_fr* omega, const b200_fr* delta, void* d_out, size_t out_stride,
+                                uint64_t* invalid, void* stream);
+
+/* ---- proving-key and SRS loading: a parameter file or a proving key straight to the device, checked there -----------------------
+ *
+ * b200_srs_register: ParamsKZG::read + ParamsKZG::downsize + two b200_bases_register_ex, in one call.  A KZG parameter file's two G1
+ * vectors go straight into registered base tables, checked on the device, with the Lagrange-basis vector computed on the device when the
+ * file is larger than the circuit.
+ * g: the first 2^k points of the file's `g` vector (G1Affine wire form, as ParamsKZG::write lays them out), in host memory; pageable
+ * memory and a memory-mapped file are both fine.  g_lagrange: the file's own 2^k-point Lagrange-basis vector, which the caller passes
+ * when the file's k equals k; NULL computes it on the device from g with the group FFT (omega^-1, then scale n^-1), as
+ * ParamsKZG::downsize does.  window_bits and max_table_bytes mean what they mean for b200_bases_register_ex and apply to both tables.
+ *
+ * Each given vector is staged through the pageable copy path straight into level 0 of its new table (no per-thread staging buffer grows
+ * to the vector's size) and every point passed is checked on the device as halo2curves' G1Affine::from_raw_bytes checks it: x and y are
+ * canonical (the 4 little-endian u64 limbs, read as a 256-bit integer, are below p) and the point is (0, 0) or satisfies y^2 = x^3 + 3.
+ * Then the Lagrange-basis vector is transformed if needed, both tables are built and copied to the other devices of the process, and
+ * *g_handle / *g_lagrange_handle receive two handles for b200_msm* and b200_bases_release.  Synchronous, like b200_bases_register.
+ *
+ * All or nothing: on any error no handle is written and no table memory is kept.  Returns -1 for bad arguments (NULL g or handle
+ * pointers, k > 26, window_bits not 0 or 4..24) before any device work, and for an invalid point, with b200_last_error() naming the
+ * vector, the index and the reason: "srs_register: g_lagrange[1234] is not on the curve" ("x is not below p", "y is not below p").
+ * With several invalid points the lowest index of g is named, else the lowest of g_lagrange.  -2 for a CUDA failure.
+ *
+ * Unlike halo2's read, only the points passed are checked: a bad point of the file beyond 2^k, or in a g_lagrange vector the caller
+ * skips because it downsizes, is never read and so never seen. */
+int b200_srs_register(const b200_g1_affine* g, const b200_g1_affine* g_lagrange, uint32_t k, int window_bits, size_t max_table_bytes,
+                      uint64_t* g_handle, uint64_t* g_lagrange_handle);
+
+/* b200_pk_load: ProvingKey::read (RawBytes, with precompute-coset) for a device-resident prover, in one call.  The Lagrange columns of a
+ * RawBytes proving key go straight into device memory, checked on the device, with the key's coefficient columns and its l0 / l_last /
+ * l_active_row cosets derived there instead of read.
+ * Inputs: h_fixed_values[j] (j < n_fixed) and h_permutations[j] (j < n_perm) are host pointers, each to one column of 2^k Fr in the
+ * key file's raw-bytes form (4 little-endian u64 Montgomery limbs, 32 B per element): the file's fixed_values and permutations
+ * sections.  They typically point into a memory-mapped key file, where they are not even 4-byte aligned (the vk prefix of the
+ * reference key is 5127 B and every column follows a u32 big-endian length), so the library treats them as byte pointers and only
+ * copies them (memcpy or a DMA copy); pageable memory is fine.  k and ext_k are the key's domain sizes (2^k rows, 2^ext_k extended
+ * rows) and blinding_factors its number of blinding rows.
+ *
+ * Outputs, all device memory owned by the caller, on one device:
+ *   d_values  the fixed columns, then the permutation columns: column c (c < n_fixed + n_perm) at element offset c * stride;
+ *   d_polys   the same columns in coefficient form (EvaluationDomain::lagrange_to_coeff), in the same layout with the same stride;
+ *   d_l       three extended columns of 2^ext_k elements back to back: l0, l_last, l_active_row.
+ * Every output is fully reduced, in Montgomery form, and byte-identical to the key's own section: fixed_values / permutations,
+ * fixed_polys / permutations.polys, and l0 / l_last / l_active_row.  Keygen's definitions apply: u = 2^k - blinding_factors - 1,
+ * l0 = L_0, l_last = L_u and l_active_row = 1 - (l_last + l_blind), where l_blind is the sum of the Lagrange polynomials of rows
+ * u + 1 ... 2^k - 1, each on the extended coset (coeff_to_extended).  The domain constants (omega, the extended omega, zeta = Fr::ZETA and
+ * 2^-k) are derived inside the library from k and ext_k.  Rows of d_values / d_polys between 2^k and stride are not written.
+ *
+ * The check: every element passed is checked as halo2curves' Fr::from_raw_bytes checks it: the four little-endian u64 limbs, read as
+ * one 256-bit integer, must be below r.  A failure returns -1 with b200_last_error() naming the section, the column and the lowest bad
+ * row, e.g. "pk_load: permutations[3][1234] is not below r"; with several bad elements the lowest (section, column, row) is named,
+ * fixed_values before permutations.  After a rejection d_polys and d_l are not written; d_values holds whatever was staged.
+ *
+ * Not read: the key's polys, cosets and l-vectors are never read, so a bad byte there is never seen.  A key whose polys disagree with
+ * its values gets the polys of its values here; halo2's keygen never writes such a key.
+ *
+ * Argument errors return -1 before any device work and write nothing: k < 1, ext_k < k, ext_k > 28, blinding_factors >= 2^k;
+ * stride < 2^k; a null pointer (d_values, d_polys and the two host arrays may be NULL when n_fixed + n_perm == 0; then only d_l is
+ * written); outputs that are not 16-byte aligned device memory of the process; outputs that overlap; outputs on different devices.
+ * -2 for a CUDA failure.
+ *
+ * Execution: on the device that owns the outputs, synchronous (the outputs are complete when the call returns), re-entrant per thread
+ * like every entry point.  No replica is made on another device.  Each column is staged through the pageable copy path straight into
+ * its slot of d_values (no per-thread staging buffer grows to the key's size) and checked right behind its copy; the check word is read
+ * back once, after the last column.
+ *
+ * Device memory held beyond the caller's buffers, by the calling thread's context (kept for its later calls, as every call's scratch
+ * is), with n = 2^k, N = 2^ext_k, C = n_fixed + n_perm and B the per-call scratch budget (B200_WS_BUDGET_MB, else a share of
+ * B200_WS_TOTAL_MB): 3 n * 32 B (the l-vectors' coefficients) and 32 * max(g n, s N) B of transform scratch, where the coefficient
+ * columns go in groups of g = min(C, 65535, max(1, floor(B / (32 n)))) columns and the l-cosets in groups of s = min(3, max(1,
+ * floor(B / (32 N)))); each buffer is allocated with 1/8 headroom, plus 8 B for the check word.  The twiddle tables of the transforms of
+ * sizes 2^k (omega^-1) and 2^ext_k (the extended omega) come on top and stay with the device.  A rejected call allocates only the check
+ * word.  The pageable copy path's two 16 MiB pinned host buffers are per thread, as for every host-pointer entry point. */
+int b200_pk_load(const void* const* h_fixed_values, size_t n_fixed, const void* const* h_permutations, size_t n_perm,
+                 uint32_t k, uint32_t ext_k, uint32_t blinding_factors,
+                 void* d_values, void* d_polys, size_t stride, void* d_l);
+
 /* ---- device / pinned memory helpers for callers without their own CUDA runtime ---------------------------------- */
 int b200_dev_alloc(void** d_ptr, size_t bytes);
 int b200_dev_alloc_on(int device_slot, void** d_ptr, size_t bytes);   /* multi-device process: allocate on device `device_slot` */

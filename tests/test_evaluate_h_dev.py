@@ -1,4 +1,4 @@
-"""b200_evaluate_h_dev (include/ezkl_b200_resident.h): the quotient from device-resident columns, one n-point coset part at a time, with the
+"""b200_evaluate_h_dev: the quotient from device-resident columns, one n-point coset part at a time, with the
 extended columns read in place.  Its result must be b200_evaluate_h's, byte for byte, on the same columns (DESIGN.md §4.4).  The checks that
 need a scratch budget run tests/evaluate_h_dev_check.py in a child process, because B200_WS_BUDGET_MB is read once, at b200_init."""
 import ctypes as C
@@ -27,17 +27,12 @@ def run_check(budget_mb, *args):
     return r.stdout
 
 
-# ---- CPU: the new header is exported and typed ---------------------------------------------------------------------------------
-def test_resident_header_is_exported_and_typed():
-    """Every prototype of include/ezkl_b200_resident.h is exported by libezkl_b200.so with the argtypes / restype read from that header, and
-    only from that header: include/ezkl_b200.h keeps its own declarations."""
-    decls = nat.declarations(nat.RESIDENT_HEADER)
-    assert set(decls) == {"b200_evaluate_h_dev"}
-    assert not set(decls) & set(nat.declarations(nat.HEADER))
-    lib = nat.lib()
-    for name, (argtypes, restype) in decls.items():
-        fn = getattr(lib, name)
-        assert fn.argtypes == argtypes and fn.restype is restype, name
+# ---- CPU: the entry point is exported and typed ---------------------------------------------------------------------------------
+def test_evaluate_h_dev_is_exported_and_typed():
+    """include/ezkl_b200.h declares b200_evaluate_h_dev, which libezkl_b200.so exports with the argtypes / restype read from that header."""
+    decls = nat.declarations(nat.HEADER)
+    fn = nat.lib().b200_evaluate_h_dev
+    assert (fn.argtypes, fn.restype) == decls["b200_evaluate_h_dev"]
     assert decls["b200_evaluate_h_dev"] == ([P, P, S, U32, U32, P, P, P, S, P, S, P, S, P, U32, P, P, P, P], Z)
 
 

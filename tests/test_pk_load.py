@@ -1,4 +1,4 @@
-"""Proving key straight to the device (include/ezkl_b200_pk.h, device.load_proving_key): the key's fixed_values and permutations columns are
+"""Proving key straight to the device (b200_pk_load, device.load_proving_key): the key's fixed_values and permutations columns are
 staged into device memory and checked there as halo2curves' Fr::from_raw_bytes checks them, and the key's coefficient columns and l-cosets are
 derived on the device instead of read.  Pinned by the reference proving key: its sections are rebuilt from tests/golden (the fixture's
 values, the fixture mapping's sigma columns, the derived sections) into a file whose sha256 is the manifest's, and the device's outputs equal
@@ -54,14 +54,9 @@ def below_r(limbs) -> bool:
 
 
 # ---- CPU ---------------------------------------------------------------------------------------------------------------------------
-def test_pk_header_is_exported_and_typed():
-    """include/ezkl_b200_pk.h declares exactly b200_pk_load, exported with the argtypes / restype read from that header and declared in no
-    other header; ezkl_b200.h keeps its 66 entry points."""
-    decls = nat.declarations(nat.PK_HEADER)
-    assert set(decls) == {"b200_pk_load"}
-    for other in (nat.HEADER, nat.RESIDENT_HEADER, nat.KEYGEN_HEADER, nat.SRS_HEADER, nat.DBG_HEADER):
-        assert not set(decls) & set(nat.declarations(other)), other
-    assert len(nat.declarations(nat.HEADER)) == 66
+def test_pk_load_is_exported_and_typed():
+    """include/ezkl_b200.h declares b200_pk_load, exported with the argtypes / restype read from that header."""
+    decls = nat.declarations(nat.HEADER)
     fn = nat.lib().b200_pk_load
     assert (fn.argtypes, fn.restype) == decls["b200_pk_load"]
     assert decls["b200_pk_load"] == ([P_, S, P_, S, U32, U32, U32, P_, P_, S, P_], Z)
